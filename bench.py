@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200-native stage-0 train step (BASELINE.json metric:
+"""bench.py -- headline benchmark of the stage-0 train step on the H100 (BASELINE.json metric:
 ray-samples/sec of one full train step, device-timed).
 
     python bench.py [--gpus N] [--steps K] [--warmup W]            # our arm (default workload: lego_stage0_converged)
@@ -8,7 +8,7 @@ ray-samples/sec of one full train step, device-timed).
     python bench.py --impl reference [--steps K] [--warmup W]      # CPU restatement of the reference step on the host cores
     torchrun --nproc-per-node N bench.py --gpus N ...              # one rank per GPU (NCCL)
 
-One "step" = one optimizer step of the fused pipeline on one batch of 4096 synthetic rays (march -> hash-grid encode -> tcgen05
+One "step" = one optimizer step of the fused pipeline on one batch of 4096 synthetic rays (march -> hash-grid encode -> wgmma
 MLPs -> composite + loss -> backward -> TV -> Adam).  `value` = samples of all ranks / max-over-ranks device time with the batch
 already resident in HBM; `e2e` = the same through Stage0Trainer.step() with pinned-host batches (H2D inside the timed region) and a
 D2H read of the loss every step.  Also in the line: `roofline` (dominant kernel, timed live with CUDA events, cold L2),
@@ -29,7 +29,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 NUM_RAYS = 4096
-ALG_BYTES = {"encode_fwd": 1053, "fwd_fused": 1053, "encode_bwd": 1024, "bwd_fused": 1024, "step": 2077}      # SURVEY.md section 8(d), bytes per sample
+ALG_BYTES = {"encode_fwd": 1053, "fwd_fused": 1053, "encode_bwd": 1024, "bwd_fused": 1024, "step": 2077}      # HBM bytes per sample the kernels must move
 
 WORKLOADS = {
     # BASELINE config 2: lego recipe (readme.md:64): bound 1, dt_gamma 0, RGBA targets + mask loss, TV 1e-8
@@ -46,23 +46,11 @@ def load_peaks():
             pk = json.load(f)
         return float(pk["hbm_gbs"]), "measured"
     except Exception:
-        return 6650.0, "fallback"
-
-
-def ncu_traffic(kernel):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of `kernel` from the committed `ncu --set full` capture of this command
-    (profiles/ncu_traffic.json, written by profiles/summarize_ncu.py), or None when that kernel was not captured."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            t = json.load(f)
-        e = t["kernels"].get(kernel)
-        return None if e is None else {"bytes": e["dram_bytes"], "capture": t.get("capture")}
-    except Exception:
-        return None
+        return 3350.0, "fallback"       # H100 SXM data-sheet HBM3 bandwidth, GB/s
 
 
 class ClockSampler(threading.Thread):
-    """SM clock and throttle reasons DURING the timed region (B200_PROFILING.md recipe).  NVML is polled in-process about every
+    """SM clock and throttle reasons DURING the timed region.  NVML is polled in-process about every
     millisecond (a timed region of a few dozen sub-millisecond steps is shorter than one `nvidia-smi -lms 100` period); if NVML
     cannot be loaded the nvidia-smi loop is the fallback."""
     REASONS = {0x8: "hw_slowdown", 0x40: "hw_thermal_slowdown", 0x20: "sw_thermal_slowdown", 0x4: "sw_power_cap"}
@@ -130,7 +118,7 @@ class ClockSampler(threading.Thread):
 
 
 # ------------------------------------------------------------------------------------------------
-# synthetic workloads (no datasets are available): SURVEY.md section 8(d)
+# synthetic workloads (no datasets are available)
 # ------------------------------------------------------------------------------------------------
 _SCENES = {}
 
@@ -180,7 +168,7 @@ def make_trainer(workload):
 
 
 # ------------------------------------------------------------------------------------------------
-# CPU arm: the repo's PyTorch restatement of the reference step (the reference has no CPU path, SURVEY.md section 8c)
+# CPU arm: the repo's PyTorch restatement of the reference step (the reference has no CPU path)
 # ------------------------------------------------------------------------------------------------
 def cpu_step_rate(steps, warmup, budget_s=150.0):
     """Times the CPU restatement of the lego train step (oracle/train_oracle.py) on a bounded sample of the 4096-ray batch: the
@@ -232,7 +220,7 @@ def cpu_baseline_dict(v, threads, rays, what):
 
 
 def run_reference(args):
-    """`--impl reference`: the reference has no CPU implementation of this path (SURVEY.md section 8c), so this arm times the
+    """`--impl reference`: the reference has no CPU implementation of this path, so this arm times the
     CPU restatement (oracle port) with the host threads that serve it best, on a bounded sample per step."""
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -291,7 +279,7 @@ def reference_cuda_leg(workload, dev_batches, state, steps=10, warmup=3):
         torch.cuda.empty_cache()
         return {"value": samples / (ms * 1e-3), "unit": "samples/s", "ms_per_step": ms / steps, "steps": steps,
                 "what": "unmodified nerf/network.py + nerf/renderer.py + nerf/utils.py (Trainer.train_step, post_train_step, "
-                        "GradScaler, torch.optim.Adam) over the reference's own CUDA kernels built for sm_100a, same batches, "
+                        "GradScaler, torch.optim.Adam) over the reference's own CUDA kernels built for sm_90a, same batches, "
                         "device-resident inputs, CUDA events"}
     except Exception as e:      # noqa: BLE001
         return {"unavailable": repr(e)[:300]}
@@ -426,6 +414,30 @@ def dp_divergence_check(workload, mode, rank, world, rays=512, steps=4):
 # ------------------------------------------------------------------------------------------------
 # our arm
 # ------------------------------------------------------------------------------------------------
+DUMP_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, tr):
+    """What the last timed step hands its caller, as DIR/<name>.npy: the loss, the number of samples marched, and every floating-point
+    tensor of the model state the step left behind (reference state_dict names).  A tensor larger than its share of the 64 MB budget is
+    written as a fixed, seeded sample of its elements (same positions for every build), so that two builds compare output for output.
+    Call it before anything that drops the prefetched batch (check_capacity, drop_prefetch): tr.cur must still be the last step's slot."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    outs = {"loss": np.array([tr.read_loss()], dtype=np.float64), "num_samples": np.array([float(tr.counters[1].item())], dtype=np.float64)}
+    state = {k: v for k, v in tr.export_reference_state().items() if v.is_floating_point()}
+    share = (DUMP_BYTES - 4096) // (4 * max(len(state), 1))
+    for k, v in state.items():
+        f = v.detach().float().reshape(-1).cpu()
+        if f.numel() > share:
+            g = torch.Generator().manual_seed(0)
+            f = f[torch.randperm(f.numel(), generator=g)[:share].sort().values]
+        outs[k] = f.numpy()
+    for k, a in outs.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
+
+
 def run_ours(args):
     import torch.distributed as dist
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -503,6 +515,8 @@ def run_ours(args):
         dist.all_reduce(samples, op=dist.ReduceOp.SUM)
     ms_total = ms.item(); samples_total = samples.item()
     value = samples_total / (ms_total * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, tr)          # before check_capacity: it drops the prefetch and moves tr.cur to the next batch
     overflow_steps, max_m = tr.check_capacity(grow=False)
 
     # ---- leg 2: end to end (pinned host -> device inside the timed region, loss read back every step) ----
@@ -538,7 +552,7 @@ def run_ours(args):
              (["bwd_fused"] if tr.fused_bwd else ["mlp_bwd", "encode_bwd"]) + ["adam"]
     acc = {s: 0.0 for s in stages}
     reps = 5
-    flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda")     # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, device="cuda")     # > 50 MB L2
     for r in range(reps):
         b = dev_batches[r % n_batches]
         tr.slots[tr.cur].load(b["ro"], b["rd"], b["gt"], b["bg"], b["noises"], b.get("cnf"))
@@ -564,10 +578,8 @@ def run_ours(args):
     dom = max(("fwd_fused" if tr.fused_fwd else "encode_fwd", "bwd_fused" if tr.fused_bwd else "encode_bwd"), key=lambda s: acc[s])
     achieved = ALG_BYTES[dom] * M_last / (acc[dom] * 1e-3) / 1e9
     kname = {"encode_fwd": "k_s0_encode_fwd", "encode_bwd": "k_s0_encode_bwd", "bwd_fused": "k_s0_bwd_fused", "fwd_fused": "k_s0_fwd_fused"}[dom]
-    traffic = ncu_traffic(kname)
     roofline = {"bound": "hbm", "kernel": kname, "achieved": achieved, "peak": peak, "peak_kind": peak_kind, "unit": "GB/s",
-                "frac": achieved / peak, "traffic": None if traffic is None else traffic["bytes"],
-                "traffic_capture": None if traffic is None else traffic["capture"], "alg_bytes_per_sample": ALG_BYTES[dom],
+                "frac": achieved / peak, "alg_bytes_per_sample": ALG_BYTES[dom],
                 "samples_per_launch": M_last, "kernel_ms": acc[dom], "stage_ms_cold_l2": {k: round(v, 4) for k, v in acc.items()},
                 "step_frac_of_hbm": ALG_BYTES["step"] * value / 1e9 / peak}
 
@@ -608,7 +620,7 @@ def run_ours(args):
                            "cuda_graph": not args.no_graph, "ray_range_parts": int(tr.nparts), "fused_bwd": bool(tr.fused_bwd), "fused_fwd": bool(tr.fused_fwd), "defer_zero": bool(tr.defer_zero), "prefetch_at": tr.prefetch_at,
                            "march_prefetch": not args.no_prefetch, **{k: v for k, v in WORKLOADS[workload].items() if k != "cap"},
                            "sample_capacity": tr.Mcap, "capacity_overflow_steps": overflow_steps, "max_samples_seen": max_m,
-                           "l2": "inputs cycle over 8 batches; tables+grads+Adam state (0.6 GB touched per step) exceed the 126 MB L2"},
+                           "l2": "inputs cycle over 8 batches; tables+grads+Adam state (0.6 GB touched per step) exceed the 50 MB L2"},
                 "clocks": clocks,
                 "e2e": {"value": e2e_value, "unit": "samples/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                         "ms_per_step": ms2.item() / K},
@@ -715,6 +727,8 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=10)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's results (loss, sample count, model state) as DIR/<name>.npy")
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="lego_stage0_converged", choices=list(WORKLOADS) + ["lego_stage1"])
     ap.add_argument("--no-graph", action="store_true")
@@ -729,7 +743,8 @@ def main():
                     help="where the next batch's march is released on the side stream: under the optimizer stage or under the forward pass")
     ap.add_argument("--defer-zero", type=int, default=1, help="1: the gradient table is zeroed on a side stream under the next step instead of by the optimizer kernel")
     ap.add_argument("--fused-fwd", type=int, default=0, help="1: gather + MLP forward as one warp-specialised launch (implies --parts 1)")
-    ap.add_argument("--fused-bwd", type=int, default=1, help="1: MLP backward + scatter as one warp-specialised launch (csrc/fused.cu)")
+    ap.add_argument("--fused-bwd", type=int, default=0, help="1: MLP backward + scatter as one warp-specialised launch (csrc/fused.cu); "
+                                                             "0: two launches, the faster choice on the H100")
     ap.add_argument("--parts", type=int, default=2, choices=[1, 2, 4, 8],
                     help="ray-range parts run as concurrent gather->MLP->composite->MLP'->scatter chains on forked streams")
     ap.add_argument("--dp", default="auto", choices=["auto", "nvls", "peer", "nccl"],
@@ -739,6 +754,8 @@ def main():
     if args.impl == "reference":
         run_reference(args)
     elif args.workload == "lego_stage1":
+        if args.dump_outputs:
+            raise SystemExit("bench.py: --dump-outputs covers the stage-0 workloads")
         run_stage1(args)
     else:
         run_ours(args)

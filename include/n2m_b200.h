@@ -1,8 +1,8 @@
-/* n2m_b200.h -- C ABI of libn2m_b200.so: the B200-native (sm_100a) replacement for the
+/* n2m_b200.h -- C ABI of libn2m_b200.so: the sm_90a (H100) replacement for the
  * native layer of nerf2mesh's stage-0 hot path.
  *
  * Every entry point replaces one function the reference binds through pybind11
- * (reference file:line given per function).  Conventions (SURVEY.md section 8b):
+ * (reference file:line given per function).  Conventions:
  *   - plain device pointers + explicit sizes, no torch types;
  *   - the CALLER allocates every output (and zero-initialises the ones marked [zero-init]);
  *     the library never allocates, frees or retains device memory and holds no state

@@ -2,7 +2,7 @@
  *
  * The operator-level entry points in n2m_b200.h are the drop-in replacements for the reference's
  * pybind functions.  The entry points here implement the same arithmetic as ONE pipeline with a
- * B200-native data layout, no host synchronisation and no per-step allocation, so the whole train
+ * GPU-native data layout, no host synchronisation and no per-step allocation, so the whole train
  * step can be captured in a CUDA graph.  What each stage replaces in the reference:
  *
  *   n2m_s0_march          raymarching.near_far_from_aabb + march_rays_train (raymarching.py:19-49,181-245;
@@ -10,10 +10,10 @@
  *   n2m_s0_encode_fwd     GridEncoder.forward x2 (grid.py:151-168; gridencoder.cu:88-196) + cat + safe_normalize
  *                          + grad_total_variation (gridencoder.cu:506-609; utils.py:801-823)
  *   n2m_s0_mlp_fwd        sigma_net / color_net / specular_net + trunc_exp / sigmoid / clamp
- *                          (nerf/network.py:81-108,159-189) on tcgen05 tensor cores
+ *                          (nerf/network.py:81-108,159-189) on wgmma tensor cores
  *   n2m_s0_composite_loss composite_rays_train fwd+bwd (raymarching.cu:501-694), background mix
  *                          (renderer.py:804) and the MSE(+mask, +specular) loss (utils.py:660-738)
- *   n2m_s0_mlp_bwd        autograd of the three MLPs (dgrad + wgrad) on tcgen05
+ *   n2m_s0_mlp_bwd        autograd of the three MLPs (dgrad + wgrad) on wgmma
  *   n2m_s0_encode_bwd     grid_encode backward x2 (gridencoder.cu:248-339)
  *   n2m_s0_adam           GradScaler.unscale_/step/update + Adam(eps 1e-15) + the per-step fp32->fp16
  *                          table cast (grid.py:45-46) + zero_grad  (utils.py:549,1163,1176-1177)
@@ -24,8 +24,8 @@
  *              64-bit access serves both encoders.  fp32 colour masters live in `color_master [rows] float2`.
  *   gtable     [rows]  float4 {g_density, g_colour0, g_colour1, 0}, loss-scaled, reduced with one
  *              red.global.add.v4.f32 per lattice corner.
- *   enc_tiles  one 16 KiB image per 128 samples: fp16 [128 x 64] in the UMMA no-swizzle core-matrix layout
- *              (chunk-major, tc05.cuh): cols 0-2 xyz, 3-18 density features, 19-50 colour features,
+ *   enc_tiles  one 16 KiB image per 128 samples: fp16 [128 x 64] in the no-swizzle core-matrix layout
+ *              (chunk-major, wg.cuh): cols 0-2 xyz, 3-18 density features, 19-50 colour features,
  *              51-53 unit view direction, 54-63 zero.  It is the A operand of every first-layer GEMM and is
  *              staged global->shared with a single bulk async copy.
  *   recs       [Mcap] float4 {t_before, dt, t_after, ray_id (bits)} per sample, ray order.
@@ -200,7 +200,7 @@ int n2m_s0_encode_bwd_part(const n2m_s0_params* p, const void* recs, const int32
                            const int32_t* offsets, void* gtable, const float* loss_scale, uint32_t part, uint32_t nparts,
                            n2m_stream_t stream);
 
-/* Fused backward (csrc/fused.cu): MLP backward (tcgen05) + hash-grid scatter of one part in ONE persistent, warp-specialised launch --
+/* Fused backward (csrc/fused.cu): MLP backward (wgmma) + hash-grid scatter of one part in ONE persistent, warp-specialised launch --
  * warps 0-3 run the MLP backward of a 128-sample tile, warps 4-19 scatter the previous tile's feature gradients, which are handed over
  * through a double-buffered shared-memory image instead of `denc_tiles` in HBM.  Same arithmetic as n2m_s0_mlp_bwd_part followed by
  * n2m_s0_encode_bwd_part (gradients equal up to fp32 atomic order); the TV gradient stays with n2m_s0_tv.  n2m_s0_fused_init sets the
@@ -298,7 +298,7 @@ int n2m_dp_adam(const void* ctx, uint32_t parity, uint32_t world, uint32_t rows,
  * table of every rank) and the refreshed 8-byte entries are broadcast with one multimem.st; mc_gtab / mc_table are the multicast addresses
  * (torch.distributed._symmetric_memory) of this parity's gradient table and of the working table.  Per rank and step the links carry 16 B x rows out
  * (the switch pulls every replica of a row once) against 16 B x rows x (W-1)/W each way with P2P loads, and the all-gather 8 B x rows / W
- * out instead of 8 B x rows x (W-1)/W: slower than n2m_dp_adam at W = 2, faster at W = 8 (profiles/r2_scaling.md).  In both entry points gtab_next / gmlp_next may be NULL: the caller then zeroes the next-parity gradient buffers itself. */
+ * out instead of 8 B x rows x (W-1)/W, so it moves fewer bytes than n2m_dp_adam for W > 4.  In both entry points gtab_next / gmlp_next may be NULL: the caller then zeroes the next-parity gradient buffers itself. */
 int n2m_dp_adam_nvls(const void* ctx, const void* mc_gtab, void* mc_table, uint32_t parity, uint32_t world, uint32_t rows, uint32_t n_mlp,
                      void* color_master_slice, float* m_slice, float* v_slice, float* mlp_params, float* m_mlp, float* v_mlp, void* wpack,
                      void* gtab_next, float* gmlp_next, float* opt_state, float eps, n2m_stream_t stream);

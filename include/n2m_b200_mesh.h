@@ -1,4 +1,4 @@
-/* n2m_b200_mesh.h -- C ABI of the stage-0 -> stage-1 mesh hand-off of libn2m_b200.so (SURVEY.md section 8 f-4).
+/* n2m_b200_mesh.h -- C ABI of the stage-0 -> stage-1 mesh hand-off of libn2m_b200.so.
  *
  * NeRFRenderer.export_stage0 (nerf/renderer.py:471-545) evaluates the density on a regular grid, copies it to the host and calls the
  * third-party PyMCubes `mcubes.marching_cubes(sigmas, density_thresh)` (:526-529; not vendored, version unpinned) before cleaning /

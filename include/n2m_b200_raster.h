@@ -1,4 +1,4 @@
-/* n2m_b200_raster.h -- C ABI of the stage-1 mesh path of libn2m_b200.so (SURVEY.md section 8 a14, BASELINE config 5).
+/* n2m_b200_raster.h -- C ABI of the stage-1 mesh path of libn2m_b200.so.
  *
  * The reference's stage 1 (NeRFRenderer.render_stage1, nerf/renderer.py:806-935) rasterizes the refined mesh with the third-party
  * nvdiffrast library and runs the colour MLPs on the covered pixels.  These entry points replace the two nvdiffrast operators on

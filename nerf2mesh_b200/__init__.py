@@ -1,4 +1,4 @@
-"""nerf2mesh_b200 -- B200-native (sm_100a) stage-0 ray-marching hot path behind nerf2mesh's
+"""nerf2mesh_b200 -- H100-native (sm_90a) stage-0 ray-marching hot path behind nerf2mesh's
 operator surface.
 
 Sub-packages `raymarching`, `gridencoder`, `shencoder` mirror the reference's modules of the

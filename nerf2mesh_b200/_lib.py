@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(_HERE, "libn2m_b200.so")
 if not os.path.exists(LIB_PATH):
     raise ImportError(
         f"{LIB_PATH} not found: build it with `python -m nerf2mesh_b200.build` "
-        "(nvcc, sm_100a). nerf2mesh_b200 has no CPU / PyTorch fallback.")
+        "(nvcc, sm_90a). nerf2mesh_b200 has no CPU / PyTorch fallback.")
 
 lib = ctypes.CDLL(LIB_PATH)
 

@@ -1,4 +1,4 @@
-"""Build libn2m_b200.so (sm_100a only) in-tree with nvcc.
+"""Build libn2m_b200.so (sm_90a only) in-tree with nvcc.
 
     python -m nerf2mesh_b200.build [--force] [--verbose]
 
@@ -18,13 +18,13 @@ LIB = os.path.join(HERE, "libn2m_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
 SOURCES = ["raymarching.cu", "gridencoder.cu", "shencoder.cu", "stage0.cu", "mlp_tc.cu", "fused.cu", "render.cu", "mcubes.cu", "raster.cu", "antialias.cu", "stage1.cu", "grid_aux.cu", "optim.cu", "dp.cu"]
-# micro-benchmarks and the tcgen05 layout probe: test / profiling infrastructure, kept OUT of the product library
-PROBE_SOURCES = ["tc_probe.cu", "red_probe.cu"]
+# micro-benchmarks and the wgmma layout probe: test / profiling infrastructure, kept OUT of the product library
+PROBE_SOURCES = ["tc_probe.cu"]
 PROBE_LIB = os.path.join(HERE, "libn2m_probes.so")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     # same numerics contract as the reference build (raymarching/backend.py:16-21):
     "-use_fast_math",
@@ -76,7 +76,7 @@ def _build(sources, LIB, link_extra, force=False, verbose=False):
                 if verbose and out.strip():
                     print(out)
     if jobs or force or not os.path.exists(LIB) or any(_newer(o, LIB) for o in objs):
-        run([NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs + link_extra)
+        run([NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs + link_extra)
     return LIB
 
 

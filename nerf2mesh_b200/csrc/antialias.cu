@@ -8,7 +8,7 @@
 // triangle that crosses strictly between the two pixel centres, if it is a silhouette edge, blends the two colours by the position
 // of the crossing: alpha = t - 0.5;  out[alpha > 0 ? Q : P] += alpha * (in[P] - in[Q]).
 //
-// B200 shape of the work (HBM / L2-atomic bound integer + fp32 work, no tensor cores):
+// Shape of the work (HBM / L2-atomic bound integer + fp32 work, no tensor cores):
 //   k_aa_topology : one thread per triangle inserts its three edges into an open-addressing hash (64-bit key (min, max) vertex,
 //                   value = the opposing vertex of up to two triangles) with atomicCAS; built once per mesh (the reference's mesh
 //                   only changes at re-meshing), 16 B per slot, load factor <= 0.5

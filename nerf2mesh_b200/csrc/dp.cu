@@ -1,11 +1,11 @@
 // dp.cu -- data-parallel optimizer step fused with its collective, over NVLink peer memory.
 //
 // With rays sharded across W GPUs every rank ends its backward pass with a full-size gradient table
-// (98 MB).  The library baseline (NCCL all-reduce of 98 MB, then a full Adam on every rank) costs
-// ~245 us of NVLink time + ~96 us of HBM streaming per step at W = 8.  This file does it as ONE pass:
+// (98 MB).  The library baseline (NCCL all-reduce of 98 MB, then a full Adam on every rank) moves the whole table over
+// NVLink and streams it through HBM on every rank.  This file does it as ONE pass:
 //
 //   reduce-scatter : rank r reads rows [r R/W, (r+1) R/W) of every peer's gradient table straight from the
-//                    peers' HBM (P2P loads over NVLink 5 / NVSwitch) and sums them,
+//                    peers' HBM (P2P loads over NVLink / NVSwitch) and sums them,
 //   optimizer      : applies GradScaler-unscale + Adam to that 1/W slice only (moments and fp32 colour
 //                    masters exist only for the slice it owns: the Adam stream shrinks W-fold),
 //   all-gather     : writes the updated 8-byte table entries into every peer's table (P2P stores),
@@ -103,7 +103,7 @@ __device__ __forceinline__ void mc_st_entry(TableEntry* mc, TableEntry e) {
 
 
 // reduce-scatter + Adam + all-gather on this rank's row slice.  All 2 x W peer loads of a thread are issued before the first use (a
-// 128-bit load over NVLink has ~2-3 us of latency; the slice is streamed with 16 of them in flight per thread).
+// 128-bit load over NVLink has microseconds of latency; the slice is streamed with 16 of them in flight per thread).
 __global__ void __launch_bounds__(256)
 k_dp_adam_tables(const DpCtx* __restrict__ ctx, uint32_t parity, float2* __restrict__ cmaster,
                  float* __restrict__ m, float* __restrict__ v, const float* __restrict__ st, float eps) {

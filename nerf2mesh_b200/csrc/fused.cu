@@ -1,19 +1,18 @@
 // fused.cu -- warp-specialised fused kernels of the stage-0 train path.
 //
-// k_s0_bwd_fused: the whole per-sample backward (autograd of the three MLPs on tcgen05 + the hash-grid scatter of
+// k_s0_bwd_fused: the whole per-sample backward (autograd of the three MLPs on wgmma + the hash-grid scatter of
 // gridencoder.cu:248-339) in ONE persistent kernel.  The stand-alone kernels (k_mlp_bwd: a latency-bound chain of ten dependent
-// tensor-core rounds per tile, 6 % occupancy; k_s0_encode_bwd: bound by the rate of spread red.global.add.v4.f32, no tensor or
-// shared-memory use) leave each other's resources idle and run back to back (122 + 179 us).  Here one CTA per SM holds
-//     warps 0-3  : the MLP backward of k_mlp_bwd, one 128-sample tile at a time (thread = sample, thread 0 issues the MMAs);
+// tensor-core rounds per tile, low occupancy; k_s0_encode_bwd: bound by the rate of spread red.global.add.v4.f32, no tensor or
+// shared-memory use) leave each other's resources idle and run back to back.  Here one CTA per SM holds
+//     warps 0-3  : the MLP backward of k_mlp_bwd, one 128-sample tile at a time (one warpgroup issuing the wgmma rounds);
 //                  the feature gradients of a finished tile go to a double-buffered shared-memory image instead of HBM,
 //     warps 4-19 : the scatter of the previous tile: warp = (32-sample group, level l mod 4), lane = sample, so consecutive lanes
 //                  are consecutive samples of a ray and runs of same-cell lanes are merged before the RED as before (the scatter is
-//                  instruction-bound at low warp counts -- 8 warps took 297 us with REDs and MMAs switched off,
-//                  profiles/fusedprobe.py -- hence sixteen warps, register budgets by setmaxnreg, lattice constants in smem),
+//                  instruction-bound at low warp counts -- see n2m_s0_set_fused_debug to time each role alone --
+//                  hence sixteen warps, register budgets by setmaxnreg, lattice constants in smem),
 // handing tiles over through two mbarrier pairs (full / empty).  The tensor chain of tile k+1 runs under the REDs of tile k, the
 // `denc_tiles` round trip through HBM (2 x 128 B per sample) disappears, and the step loses one launch per part.
 #include "n2m_common.cuh"
-#include "tc05.cuh"
 #include "s0_geom.cuh"
 #include "mlp_common.cuh"
 #include "../../include/n2m_b200_fused.h"
@@ -23,8 +22,10 @@ namespace {
 
 constexpr uint32_t kMlpThreads = 128, kScatWarps = 16, kFusedThreads = kMlpThreads + 32 * kScatWarps;     // 640
 // register budget (setmaxnreg, multiples of 8).  The kernel starts with 96 registers per thread; setmaxnreg.inc can only take what
-// setmaxnreg.dec of the other warps returned to the CTA pool: 512 x (96 - 72) = 12 288 >= 128 x (184 - 96) = 11 264.  (200 for the
-// MLP warps asked for more than the pool held: the inc never completed and the hand-over barriers timed out.)
+// setmaxnreg.dec of the other warps returned to the CTA pool: 512 x (96 - 72) = 12 288 >= 128 x (184 - 96) = 11 264.
+// ptxas (CUDA 12.9, sm_90a) compiles this 640-thread kernel at 96 registers per thread whatever these budgets say, and the MLP
+// warps' wgmma accumulators (120 weight-gradient registers beside a layer's 64) spill: 960 B of stack, about 1.5 KB of spill
+// stores per thread (-Xptxas -v).  That is why the two-launch backward (k_mlp_bwd + k_s0_encode_bwd) is the default (stage0.py).
 constexpr uint32_t kMlpRegs = 184, kScatRegs = 72;
 static_assert(kScatWarps * 32 * (96 - kScatRegs) >= kMlpThreads * (kMlpRegs - 96), "setmaxnreg.inc must fit in what setmaxnreg.dec releases");
 constexpr uint32_t D_CHUNKS = 7;                          // gradient columns 0..55 (cols 3..50 are used)
@@ -33,15 +34,13 @@ constexpr uint32_t FB_DENC = B_BYTES;
 constexpr uint32_t FB_BYTES = B_BYTES + 2 * D_BYTES;      // 168960
 
 __device__ __forceinline__ void bar_mlp() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-// MLP warps only: make generic smem writes visible to the tensor core, order TMEM accesses, meet at named barrier 1
+// MLP warps only: make generic smem writes visible to the tensor core, meet at named barrier 1
 __device__ __forceinline__ void sync_mlp() {
-    tc::fence_async_smem();
-    tc::fence_before_sync();
+    wg::fence_async_smem();
     bar_mlp();
-    tc::fence_after_sync();
 }
 __device__ __forceinline__ void mbar_arrive1(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(tc::smem_u32(bar)) : "memory");
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(wg::smem_u32(bar)) : "memory");
 }
 
 // per-level lattice constants, computed once per CTA into shared memory (level_geom + the dense / hashed index decision of
@@ -139,8 +138,7 @@ k_s0_bwd_fused(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const flo
                float4* __restrict__ gtable, float* __restrict__ g_mlp, float* __restrict__ loss_scale, uint32_t part, uint32_t nparts,
                uint32_t dbg) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint64_t bar_mma, bar_tma, bar_full[2], bar_empty[2];
-    __shared__ uint32_t tmem_s;
+    __shared__ uint64_t bar_tma, bar_full[2], bar_empty[2];
     __shared__ LevelConst s_lc[kLevels];
     const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const PartRange pr = part_range(counters, part, nparts);
@@ -149,38 +147,19 @@ k_s0_bwd_fused(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const flo
     if (pr.hi <= pr.lo || t0 + blockIdx.x >= t1) return;
 
     if (tid == 0) {
-        tc::mbar_init(&bar_mma, 1); tc::mbar_init(&bar_tma, 1);
-        tc::mbar_init(&bar_full[0], 1); tc::mbar_init(&bar_full[1], 1);
-        tc::mbar_init(&bar_empty[0], kScatWarps); tc::mbar_init(&bar_empty[1], kScatWarps);
-        tc::mbar_init_fence();
+        wg::mbar_init(&bar_tma, 1);
+        wg::mbar_init(&bar_full[0], 1); wg::mbar_init(&bar_full[1], 1);
+        wg::mbar_init(&bar_empty[0], kScatWarps); wg::mbar_init(&bar_empty[1], kScatWarps);
+        wg::mbar_init_fence();
     }
-    if (warp == 0) tc::tmem_alloc(&tmem_s, 512);
     if (tid >= kMlpThreads && tid < kMlpThreads + kLevels) s_lc[tid - kMlpThreads] = make_level_const(offsets, tid - kMlpThreads, p.S, p.base_res);
     for (uint32_t i = tid; i < W_BYTES / 16; i += kFusedThreads)
         reinterpret_cast<uint4*>(smem + B_W)[i] = __ldg(reinterpret_cast<const uint4*>(wpack) + i);
-    uint8_t* sW = smem + B_W; uint8_t* act = smem + B_ACT; uint8_t* grd = smem + B_GRAD;
-    uint8_t* sA = act + A_A; uint8_t* sH2 = act + A_H2; uint8_t* sH1 = act + A_H1; uint8_t* sS1 = act + A_S1;
-    uint8_t* sP1 = act + A_P1; uint8_t* sAs2 = act + A_AS2;
-    uint8_t* sdH = grd + G_DH; uint8_t* sdS1 = grd + G_DS1; uint8_t* sdP1 = grd + G_DP1; uint8_t* sdO = grd + G_DO;
-    uint8_t* sdOs = grd + G_DOS; uint8_t* sdO2 = grd + G_DO2;
+    uint8_t* sA = smem + B_ACT + A_A;
     uint8_t* sD = smem + FB_DENC;
-    if (tid < kMlpThreads) {   // constant-zero parts of the narrow tiles (their second K chunk, and unused columns of the first)
-        const uint4 z = make_uint4(0, 0, 0, 0);
-        *reinterpret_cast<uint4*>(sAs2 + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdO + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdOs + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdO2 + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sAs2 + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sP1 + tid * 16) = z; *reinterpret_cast<uint4*>(sP1 + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sP1 + 2 * kChunk + tid * 16) = z; *reinterpret_cast<uint4*>(sP1 + 3 * kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdP1 + tid * 16) = z; *reinterpret_cast<uint4*>(sdP1 + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdP1 + 2 * kChunk + tid * 16) = z; *reinterpret_cast<uint4*>(sdP1 + 3 * kChunk + tid * 16) = z;
-    }
-    tc::fence_async_smem();
-    tc::fence_before_sync();
+    if (tid < kMlpThreads) zero_narrow_tiles(smem, tid);
+    wg::fence_async_smem();
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = tmem_s;
 
     if (warp >= 4) {
         // =========================================== scatter warps ===========================================
@@ -199,7 +178,7 @@ k_s0_bwd_fused(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const flo
             } else {
                 s.x = s.y = s.z = s.u = s.v = s.w = 0.5f; s.dx = s.dy = s.dz = 0.f;
             }
-            tc::mbar_wait(&bar_full[buf], use & 1);
+            wg::mbar_wait(&bar_full[buf], use & 1);
             const uint8_t* row = sD + buf * D_BYTES + r * 16;
             if (lq == 0 && active) {   // fp16 overflow of the loss-scaled gradients => GradScaler semantics: flag, the step is skipped
                 bool bad = false;
@@ -224,19 +203,18 @@ k_s0_bwd_fused(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const flo
     } else {
         // =========================================== MLP warps (k_mlp_bwd) ===========================================
         asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(kMlpRegs));
-        const uint32_t lane_t = (warp * 32u) << 16;
-        const uint32_t K0 = tmem + T_K0, K1 = tmem + T_K1;
-        uint32_t ph_mma = 0, ph_tma = 0;
+        uint32_t ph_tma = 0;
         const bool full = p.shading_full != 0;
         const float ls = loss_scale[0];
         const float spec_reg = (M > 0) ? 2.0f * p.lambda_specular / (float)M * ls : 0.f;
-        bool first = true;
-        const tc::Operand G1 = opMN(sA, 128), G2 = opMN(sH2, 128), G3 = opMN(sS1, 128);
+        const uint32_t r = sample_row(tid);
+        WgradAcc wa;
+        wa.zero();
         uint32_t it = 0;
         for (uint32_t tile = t0 + blockIdx.x; tile < t1; tile += gridDim.x, ++it) {
             const uint32_t buf = it & 1, use = it >> 1;
             if (dbg & 2u) {          // probe mode: no tensor-core work, hand a zero image over at once (measures the scatter warps alone)
-                tc::mbar_wait(&bar_empty[buf], (use & 1) ^ 1);
+                wg::mbar_wait(&bar_empty[buf], (use & 1) ^ 1);
 #pragma unroll
                 for (uint32_t ch = 0; ch < D_CHUNKS; ++ch) *reinterpret_cast<uint4*>(sD + buf * D_BYTES + ch * kChunk + tid * 16) = make_uint4(0x3c003c00u, 0x3c003c00u, 0x3c003c00u, 0x3c003c00u);
                 bar_mlp();
@@ -244,251 +222,42 @@ k_s0_bwd_fused(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const flo
                 continue;
             }
             if (tid == 0) bulk_g2s(sA, enc_tiles + (size_t)tile * kTileBytes, kTileBytes, &bar_tma);
-            const uint32_t j = tile * kTile + tid;
+            const uint32_t j = tile * kTile + r;
             float4 dv = make_float4(0.f, 0.f, 0.f, 0.f);
             const bool own = j >= pr.lo && j < pr.hi;
             if (own) dv = dout[j];
-            tc::mbar_wait(&bar_tma, ph_tma); ph_tma ^= 1;
-
-            // ---------------- forward recompute ----------------
-            if (tid == 0) {
-                tc::gemm_issue(K0, opK(sA, 128), opK(sW + W_C1, 64), 128, 64, 64, false);
-                tc::gemm_issue(K1, opK(sA, 128), opK(sW + W_S1, 32), 128, 32, 64, false);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            epi_store_row<64, true>(K0 + lane_t, sH1, tid, nullptr);
-            epi_store_row<32, true>(K1 + lane_t, sS1, tid, nullptr);
-            sync_mlp();
-            if (tid == 0) {
-                tc::gemm_issue(K0, opK(sH1, 128), opK(sW + W_C2, 64), 128, 64, 64, false);
-                tc::gemm_issue(K1, opK(sS1, 128), opK(sW + W_S2, 16), 128, 16, 32, false);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            float h_sig;
-            { float v[8]; tc::tmem_ld8(K1 + lane_t, v); h_sig = round_h(v[0]); }
-            epi_store_row<64, true>(K0 + lane_t, sH2, tid, nullptr);
-            sync_mlp();
-            if (tid == 0) {
-                tc::gemm_issue(K0, opK(sH2, 128), opK(sW + W_C3, 16), 128, 16, 64, false);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            float feat[6];
-            { float v[8]; tc::tmem_ld8(K0 + lane_t, v);
+            wg::mbar_wait(&bar_tma, ph_tma); ph_tma ^= 1;
+            mlp_bwd_tile(smem, dv, own, full, spec_reg, tid, wa, sync_mlp, [&](const float (&d)[2][32]) {
+                // the scatter warps must have taken the buffer's previous contents (two tiles ago) before it is overwritten
+                wg::mbar_wait(&bar_empty[buf], (use & 1) ^ 1);
+                // the feature gradients -> the shared-memory gradient image (zeros for rows of other parts)
+                uint8_t* dst = sD + buf * D_BYTES;
 #pragma unroll
-              for (int i = 0; i < 6; ++i) feat[i] = sigmoid_h(v[i]); }
-            float sp[3] = {0.f, 0.f, 0.f};
-            if (full) {
-                const uint4 dq = *reinterpret_cast<const uint4*>(sA + 6 * kChunk + tid * 16);
-                const __half2 d01 = *reinterpret_cast<const __half2*>(&dq.y);
-                const __half2 d23 = *reinterpret_cast<const __half2*>(&dq.z);
-                const float in[8] = {__high2float(d01), __low2float(d23), __high2float(d23), feat[3], feat[4], feat[5], 0.f, 0.f};
-                store_chunk(sAs2, 0, tid, in);
-                sync_mlp();
-                if (tid == 0) {
-                    tc::gemm_issue(K1, opK(sAs2, 128), opK(sW + W_P1, 32), 128, 32, 16, false);
-                    tc::mma_commit(&bar_mma);
-                }
-                tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-                epi_store_row<32, true>(K1 + lane_t, sP1, tid, nullptr);
-                sync_mlp();
-                if (tid == 0) {
-                    tc::gemm_issue(K0, opK(sP1, 128), opK(sW + W_P2, 16), 128, 16, 32, false);
-                    tc::mma_commit(&bar_mma);
-                }
-                tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-                float v[8];
-                tc::tmem_ld8(K0 + lane_t, v);
+                for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-                for (int i = 0; i < 3; ++i) sp[i] = sigmoid_h(v[i]);
-            }
-
-            // ---------------- output-side chain rule (thread-per-sample) ----------------
-            float dfeat[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-            {
-                const float dcol[3] = {dv.y, dv.z, dv.w};
-                float dO2[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-                for (int c = 0; c < 3; ++c) {
-                    float g = dcol[c];
-                    if (full) {
-                        const float cs = round_h(sp[c] + feat[c]);
-                        if (!(cs >= 0.f && cs <= 1.f)) g = 0.f;            // clamp(0,1) backward
-                        const float dsp = own ? g + spec_reg * sp[c] : 0.f;
-                        dO2[c] = dsp * sp[c] * (1.0f - sp[c]);            // sigmoid backward
+                    for (int i = 0; i < 4 * (int)D_CHUNKS; i += 2) {
+                        const uint32_t row = frag_row(hh, i, tid), jr = tile * kTile + row;
+                        const bool mine = jr >= pr.lo && jr < pr.hi;
+                        *reinterpret_cast<uint32_t*>(dst + wg::tile_off(row, frag_col(i, tid), kTile)) = mine ? pack2(d[hh][i], d[hh][i + 1]) : 0u;
                     }
-                    dfeat[c] = g;
-                }
-                float dOs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-                dOs[0] = dv.x * __expf(fminf(fmaxf(h_sig, -15.f), 15.f));   // trunc_exp backward (activation.py:13-17)
-                store_chunk(sdOs, 0, tid, dOs);
-                if (full) store_chunk(sdO2, 0, tid, dO2);
-            }
-            sync_mlp();
-
-            // ---------------- B1 ----------------
-            if (tid == 0) {
-                tc::gemm_issue(K0, opK(sdOs, 128), opMN(sW + W_S2, 16), 128, 32, 16, false);
-                tc::gemm_issue(tmem + T_S2, G3, opMN(sdOs, 128), 128, 16, 128, !first);
-                if (full) {
-                    tc::gemm_issue(K1, opK(sdO2, 128), opMN(sW + W_P2, 16), 128, 32, 16, false);
-                    tc::gemm_issue(tmem + T_P2, G3, opMN(sdO2, 128), 128, 16, 128, !first);
-                }
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            epi_store_row<32, false>(K0 + lane_t, sdS1, tid, sS1);
-            if (full) epi_store_row<32, false>(K1 + lane_t, sdP1, tid, sP1);
-            sync_mlp();
-
-            // ---------------- B2 ----------------
-            if (tid == 0) {
-                tc::gemm_issue(K0, opK(sdS1, 128), opMN(sW + W_S1, 32), 128, 64, 32, false);
-                tc::gemm_issue(tmem + T_S1, G1, opMN(sdS1, 128), 128, 32, 128, !first);
-                if (full) {
-                    tc::gemm_issue(K1, opK(sdP1, 128), opMN(sW + W_P1, 32), 128, 16, 32, false);
-                    tc::gemm_issue(tmem + T_P1, G3, opMN(sdP1, 128), 128, 32, 128, !first);
-                }
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            {
-                if (full) {
-                    float v[8];
-                    tc::tmem_ld8(K1 + lane_t, v);
-                    dfeat[3] = v[3]; dfeat[4] = v[4]; dfeat[5] = v[5];
-                }
-                float dO[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-                for (int i = 0; i < 6; ++i) dO[i] = dfeat[i] * feat[i] * (1.0f - feat[i]);
-                store_chunk(sdO, 0, tid, dO);
-            }
-            sync_mlp();
-
-            // ---------------- B3 ----------------
-            if (tid == 0) {
-                tc::gemm_issue(K1, opK(sdO, 128), opMN(sW + W_C3, 16), 128, 64, 16, false);
-                tc::gemm_issue(tmem + T_C3, G2, opMN(sdO, 128), 128, 16, 128, !first);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            epi_store_row<64, false>(K1 + lane_t, sdH, tid, sH2);
-            sync_mlp();
-
-            // ---------------- B4 ----------------
-            if (tid == 0) {
-                tc::gemm_issue(K1, opK(sdH, 128), opMN(sW + W_C2, 64), 128, 64, 64, false);
-                tc::gemm_issue(tmem + T_C2, G2, opMN(sdH, 128), 128, 64, 128, !first);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            epi_store_row<64, false>(K1 + lane_t, sdH, tid, sH1);
-            sync_mlp();
-
-            // ---------------- B5 ----------------
-            if (tid == 0) {
-                tc::gemm_issue(K0, opK(sdH, 128), opMN(sW + W_C1, 64), 128, 64, 64, true);
-                tc::gemm_issue(tmem + T_C1, G1, opMN(sdH, 128), 128, 64, 128, !first);
-                tc::mma_commit(&bar_mma);
-            }
-            // the scatter warps must have taken the buffer's previous contents (two tiles ago) before it is overwritten
-            tc::mbar_wait(&bar_empty[buf], (use & 1) ^ 1);
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            {   // this sample's feature gradients -> its row of the shared-memory gradient image (zeros for rows of other parts)
-                uint8_t* dst = sD + buf * D_BYTES + tid * 16;
-#pragma unroll
-                for (int c0 = 0; c0 < 64; c0 += 16) {
-                    float v[16];
-                    tc::tmem_ld16(K0 + lane_t + c0, v);
-#pragma unroll
-                    for (int qq = 0; qq < 2; ++qq) {
-                        if (c0 / 8 + qq >= (int)D_CHUNKS) continue;
-                        uint4 o;
-                        o.x = pack2(v[8 * qq + 0], v[8 * qq + 1]); o.y = pack2(v[8 * qq + 2], v[8 * qq + 3]);
-                        o.z = pack2(v[8 * qq + 4], v[8 * qq + 5]); o.w = pack2(v[8 * qq + 6], v[8 * qq + 7]);
-                        if (!own) o = make_uint4(0, 0, 0, 0);
-                        *reinterpret_cast<uint4*>(dst + (c0 / 8 + qq) * kChunk) = o;
-                    }
-                }
-            }
-            first = false;
-            sync_mlp();          // every row of the image is written, all reads of this tile's smem / TMEM are done
+            });
+            sync_mlp();          // every row of the image is written, all reads of this tile's smem are done
             if (tid == 0) mbar_arrive1(&bar_full[buf]);
         }
-
-        // ---------------- flush the weight-gradient accumulators (one row of each per thread) ----------------
-        {
-            const uint32_t i = tid;
-            float v[16];
-            {
-                const int k = i < 64 ? map_c1(i) : -1;
-#pragma unroll
-                for (int c0 = 0; c0 < 64; c0 += 16) {
-                    tc::tmem_ld16(tmem + T_C1 + lane_t + c0, v);
-                    if (k >= 0) {
-#pragma unroll
-                        for (int o = 0; o < 16; ++o) atomicAdd(g_mlp + P_C0 + (c0 + o) * 35 + k, v[o]);
-                    }
-                }
-            }
-#pragma unroll
-            for (int c0 = 0; c0 < 64; c0 += 16) {
-                tc::tmem_ld16(tmem + T_C2 + lane_t + c0, v);
-                if (i >= 64) {
-#pragma unroll
-                    for (int o = 0; o < 16; ++o) atomicAdd(g_mlp + P_C1 + (c0 + o) * 64 + (i - 64), v[o]);
-                }
-            }
-            tc::tmem_ld16(tmem + T_C3 + lane_t, v);
-            if (i < 64) {
-#pragma unroll
-                for (int o = 0; o < 6; ++o) atomicAdd(g_mlp + P_C2 + o * 64 + i, v[o]);
-            }
-#pragma unroll
-            for (int c0 = 0; c0 < 32; c0 += 16) {
-                tc::tmem_ld16(tmem + T_S1 + lane_t + c0, v);
-                const int k = i < 64 ? map_s1(i) : -1;
-                if (k >= 0) {
-#pragma unroll
-                    for (int o = 0; o < 16; ++o) atomicAdd(g_mlp + P_S0 + (c0 + o) * 19 + k, v[o]);
-                }
-            }
-            tc::tmem_ld16(tmem + T_S2 + lane_t, v);
-            if (i < 32) atomicAdd(g_mlp + P_S1 + i, v[0]);
-            if (full) {
-                tc::tmem_ld16(tmem + T_P2 + lane_t, v);
-                if (i >= 32 && i < 64) {
-#pragma unroll
-                    for (int o = 0; o < 3; ++o) atomicAdd(g_mlp + P_P1 + o * 32 + (i - 32), v[o]);
-                }
-#pragma unroll
-                for (int c0 = 0; c0 < 32; c0 += 16) {
-                    tc::tmem_ld16(tmem + T_P1 + lane_t + c0, v);
-                    if (i >= 64 && i < 70) {
-#pragma unroll
-                        for (int o = 0; o < 16; ++o) atomicAdd(g_mlp + P_P0 + (c0 + o) * 6 + (i - 64), v[o]);
-                    }
-                }
-            }
-        }
+        flush_wgrad(wa, g_mlp, full, tid);
     }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem, 512);
 }
 
 
 // ================================================================================================================================
 // k_s0_fwd_fused: hash-grid gather + the three MLPs' forward in ONE persistent kernel (north_star's "fused march+encode+MLP"; the march
 // itself stays a separate, prefetched launch: it does not depend on the parameters and runs under the previous step).
-//   warps 0-3   : the MLP forward of k_mlp_fwd on the tile image in shared memory (thread = sample, thread 0 issues the tcgen05.mma rounds),
+//   warps 0-3   : the MLP forward of k_mlp_fwd on the tile image in shared memory (one warpgroup issuing the wgmma rounds),
 //   warps 4-7   : gather group 0, warps 8-11: gather group 1.  A group gathers one 128-sample tile (thread = sample, all 16 levels: the
-//                 code of the stand-alone gather), writes the UMMA-layout rows straight into ITS shared-memory buffer -- the image never
+//                 code of the stand-alone gather), writes the core-matrix-layout rows straight into ITS shared-memory buffer -- the image never
 //                 makes the HBM round trip -- and has the TMA unit store a copy to `enc_tiles` for the backward pass (cp.async.bulk
 //                 shared -> global, 16 KiB per instruction).
-// Two CTAs per SM (86 KB of shared memory, 128 TMEM columns, 85 registers each): 16 gather warps per SM keep the L1 / L2 gather pipe
+// Two CTAs per SM (86 KB of shared memory, 80 registers per thread each): 16 gather warps per SM keep the L1 / L2 gather pipe
 // busy while two tensor-core chains run underneath.  Whole-batch only (nparts == 1): the bulk store writes complete tiles.
 // ================================================================================================================================
 constexpr uint32_t kFwdThreads = 384;
@@ -505,8 +274,7 @@ k_s0_fwd_fused(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* 
                const float* __restrict__ rays_d, const TableEntry* __restrict__ table, const int32_t* __restrict__ offsets,
                const uint8_t* __restrict__ wpack, uint8_t* __restrict__ enc_tiles, float4* __restrict__ out, float* __restrict__ spec_sq_sum) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint64_t bar_mma, bar_full[2], bar_empty[2];
-    __shared__ uint32_t tmem_s;
+    __shared__ uint64_t bar_full[2], bar_empty[2];
     __shared__ float red[4];
     const uint32_t tid = threadIdx.x, warp = tid >> 5;
     const PartRange pr = part_range(counters, 0, 1);
@@ -515,19 +283,15 @@ k_s0_fwd_fused(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* 
     const uint32_t my_tiles = (t1 - blockIdx.x + gridDim.x - 1) / gridDim.x;        // tiles blockIdx.x, + gridDim.x, ...
 
     if (tid == 0) {
-        tc::mbar_init(&bar_mma, 1);
-        tc::mbar_init(&bar_full[0], 1); tc::mbar_init(&bar_full[1], 1);
-        tc::mbar_init(&bar_empty[0], 1); tc::mbar_init(&bar_empty[1], 1);
-        tc::mbar_init_fence();
+        wg::mbar_init(&bar_full[0], 1); wg::mbar_init(&bar_full[1], 1);
+        wg::mbar_init(&bar_empty[0], 1); wg::mbar_init(&bar_empty[1], 1);
+        wg::mbar_init_fence();
     }
-    if (warp == 0) tc::tmem_alloc(&tmem_s, 128);
     for (uint32_t i = tid; i < W_BYTES / 16; i += kFwdThreads)
         reinterpret_cast<uint4*>(smem + FF_W)[i] = __ldg(reinterpret_cast<const uint4*>(wpack) + i);
     if (tid < 128) *reinterpret_cast<uint4*>(smem + FF_AS2 + kChunk + tid * 16) = make_uint4(0, 0, 0, 0);     // second K chunk of the specular input: zero
-    tc::fence_async_smem();
-    tc::fence_before_sync();
+    wg::fence_async_smem();
     __syncthreads();
-    tc::fence_after_sync();
 
     if (warp >= 4) {
         // =========================================== gather groups ===========================================
@@ -541,15 +305,15 @@ k_s0_fwd_fused(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* 
             // the buffer is free once the TMA store of its previous image has read it and the MLP warps are done with that tile
             if (r == 0) {
                 asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                tc::mbar_wait(&bar_empty[g], (k & 1) ^ 1);
+                wg::mbar_wait(&bar_empty[g], (k & 1) ^ 1);
             }
             bar_group(g);
             store_tile_row(buf, r, feat);
-            tc::fence_async_smem();                  // generic-proxy writes -> visible to the tensor core and to the bulk copy engine
+            wg::fence_async_smem();                  // generic-proxy writes -> visible to the tensor core and to the bulk copy engine
             bar_group(g);
             if (r == 0) {
                 asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
-                             :: "l"(enc_tiles + (size_t)tile * kTileBytes), "r"(tc::smem_u32(buf)), "r"(kTileBytes) : "memory");
+                             :: "l"(enc_tiles + (size_t)tile * kTileBytes), "r"(wg::smem_u32(buf)), "r"(kTileBytes) : "memory");
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
                 mbar_arrive1(&bar_full[g]);
             }
@@ -557,98 +321,21 @@ k_s0_fwd_fused(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* 
         if (r == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");        // the last stores complete before the CTA exits
     } else {
         // =========================================== MLP warps (k_mlp_fwd) ===========================================
-        const uint32_t tmem = tmem_s, D0 = tmem, D1 = tmem + 64;
-        const uint32_t lane_t = (warp * 32u) << 16;
-        uint32_t ph_mma = 0;
         float spec_sq = 0.f;
-        uint8_t* sW = smem + FF_W; uint8_t* sH = smem + FF_H; uint8_t* sS1 = smem + FF_S1; uint8_t* sP1 = smem + FF_S1;
-        uint8_t* sAs2 = smem + FF_AS2;
-        const tc::OpDesc dA0 = tc::make_opdesc(opK(smem + FF_A0, 128)), dA1 = tc::make_opdesc(opK(smem + FF_A1, 128)),
-                         dH = tc::make_opdesc(opK(sH, 128)), dS1 = tc::make_opdesc(opK(sS1, 128)), dP1 = tc::make_opdesc(opK(sP1, 128)),
-                         dAs2 = tc::make_opdesc(opK(sAs2, 128));
-        const tc::OpDesc wC1 = tc::make_opdesc(opK(sW + W_C1, 64)), wC2 = tc::make_opdesc(opK(sW + W_C2, 64)),
-                         wC3 = tc::make_opdesc(opK(sW + W_C3, 16)), wS1 = tc::make_opdesc(opK(sW + W_S1, 32)),
-                         wS2 = tc::make_opdesc(opK(sW + W_S2, 16)), wP1 = tc::make_opdesc(opK(sW + W_P1, 32)),
-                         wP2 = tc::make_opdesc(opK(sW + W_P2, 16));
+        const uint32_t r = sample_row(tid);
         for (uint32_t it = 0; it < my_tiles; ++it) {
             const uint32_t tile = blockIdx.x + it * gridDim.x, g = it & 1;
             const uint8_t* sA = smem + (g ? FF_A1 : FF_A0);
-            const tc::OpDesc& dA = g ? dA1 : dA0;
-            tc::mbar_wait(&bar_full[g], (it >> 1) & 1);
-            tc::fence_after_sync();
-            // round 1: first layers of color_net and sigma_net
-            if (tid == 0) {
-                tc::gemm_issue_fast<64, 4, false, false>(D0, dA, wC1, false);
-                tc::gemm_issue_fast<32, 4, false, false>(D1, dA, wS1, false);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            epi_store_row<64, true>(D0 + lane_t, sH, tid, nullptr);
-            epi_store_row<32, true>(D1 + lane_t, sS1, tid, nullptr);
-            sync_mlp();
-            // round 2: color_net.1, sigma_net.1
-            if (tid == 0) {
-                tc::gemm_issue_fast<64, 4, false, false>(D0, dH, wC2, false);
-                tc::gemm_issue_fast<16, 2, false, false>(D1, dS1, wS2, false);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            float sigma;
-            {
-                float v[8];
-                tc::tmem_ld8(D1 + lane_t, v);
-                sigma = __expf(round_h(v[0]));                 // trunc_exp forward (activation.py:5-11)
-            }
-            epi_store_row<64, true>(D0 + lane_t, sH, tid, nullptr);
-            sync_mlp();
-            // round 3: color_net.2
-            if (tid == 0) {
-                tc::gemm_issue_fast<16, 4, false, false>(D0, dH, wC3, false);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            float feat[6];
-            {
-                float v[8];
-                tc::tmem_ld8(D0 + lane_t, v);
-#pragma unroll
-                for (int i = 0; i < 6; ++i) feat[i] = sigmoid_h(v[i]);
-            }
-            float cr = feat[0], cg = feat[1], cb = feat[2];
-            float sp[3] = {0.f, 0.f, 0.f};
-            if (p.shading_full) {
-                const uint4 dq = *reinterpret_cast<const uint4*>(sA + 6 * kChunk + tid * 16);
-                const __half2 d01 = *reinterpret_cast<const __half2*>(&dq.y);
-                const __half2 d23 = *reinterpret_cast<const __half2*>(&dq.z);
-                const float in[8] = {__high2float(d01), __low2float(d23), __high2float(d23), feat[3], feat[4], feat[5], 0.f, 0.f};
-                store_chunk(sAs2, 0, tid, in);
-                sync_mlp();
-                if (tid == 0) {
-                    tc::gemm_issue_fast<32, 1, false, false>(D1, dAs2, wP1, false);
-                    tc::mma_commit(&bar_mma);
-                }
-                tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-                epi_store_row<32, true>(D1 + lane_t, sP1, tid, nullptr);
-                sync_mlp();
-                if (tid == 0) {
-                    tc::gemm_issue_fast<16, 2, false, false>(D0, dP1, wP2, false);
-                    tc::mma_commit(&bar_mma);
-                }
-                tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-                float v[8];
-                tc::tmem_ld8(D0 + lane_t, v);
-#pragma unroll
-                for (int i = 0; i < 3; ++i) sp[i] = sigmoid_h(v[i]);
-                cr = fminf(fmaxf(round_h(sp[0] + cr), 0.f), 1.f);
-                cg = fminf(fmaxf(round_h(sp[1] + cg), 0.f), 1.f);
-                cb = fminf(fmaxf(round_h(sp[2] + cb), 0.f), 1.f);
-            }
-            const uint32_t j = tile * kTile + tid;
+            wg::mbar_wait(&bar_full[g], (it >> 1) & 1);
+            float sp[3];
+            const float4 o = mlp_fwd_tile(sA, smem + FF_W, smem + FF_H, smem + FF_S1, smem + FF_S1, smem + FF_AS2, p.shading_full != 0,
+                                          tid, sp, sync_mlp);
+            const uint32_t j = tile * kTile + r;
             if (j < pr.hi) {
-                out[j] = make_float4(sigma, cr, cg, cb);
+                out[j] = o;
                 spec_sq += sp[0] * sp[0] + sp[1] * sp[1] + sp[2] * sp[2];
             }
-            sync_mlp();                                   // every read of this tile's image / TMEM columns is done
+            sync_mlp();                                   // every read of this tile's image is done
             if (tid == 0) mbar_arrive1(&bar_empty[g]);
         }
 #pragma unroll
@@ -657,9 +344,6 @@ k_s0_fwd_fused(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* 
         bar_mlp();
         if (tid == 0 && spec_sq_sum) atomicAdd(spec_sq_sum, red[0] + red[1] + red[2] + red[3]);
     }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem_s, 128);
 }
 
 }  // namespace
@@ -671,14 +355,14 @@ static uint32_t g_fused_dbg = 0;
 
 static int fused_num_sms() {
     static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
+    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
     return n;
 }
 
 extern "C" {
 
 /* profiling hook: bit 0 = the scatter warps skip their REDs, bit 1 = the MLP warps skip the tensor-core rounds (results are then
- * meaningless; used by profiles/ to time each role of the fused backward alone) */
+ * meaningless; used to time each role of the fused backward alone) */
 int n2m_s0_set_fused_debug(int mode) { g_fused_dbg = (uint32_t)mode; return 0; }
 
 int n2m_s0_fused_init(void) {

@@ -1,4 +1,4 @@
-// gridencoder.cu -- multiresolution hash / tiled grid encoding for sm_100a (unfused operator form).
+// gridencoder.cu -- multiresolution hash / tiled grid encoding for sm_90a (unfused operator form).
 //
 // Replaces the native layer behind the reference's `grid_encode` / `GridEncoder`
 // (reference: gridencoder/src/gridencoder.cu).  Level geometry, corner order, hashing and the

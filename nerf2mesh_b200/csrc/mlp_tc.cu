@@ -1,18 +1,18 @@
 // mlp_tc.cu -- the three tiny MLPs of NeRFNetwork (nerf/network.py:66-189) forward and backward on
-// Blackwell tensor cores: hand-written tcgen05.mma (kind::f16, fp16 operands, fp32 accumulation in
-// TMEM), operands staged in shared memory as UMMA core-matrix tiles, first-layer activations brought
+// Hopper tensor cores: hand-written wgmma (m64nNk16, fp16 operands from shared memory, fp32 accumulation
+// in registers), operands staged in shared memory as core-matrix tiles, first-layer activations brought
 // in with one bulk async copy (TMA unit, cp.async.bulk) per 128-sample tile.
 //
-// Mapping: one CTA = 128 threads = one 128-sample tile = the M dimension of every forward / dgrad
-// GEMM; tcgen05.ld in the 32x32b shape hands thread t exactly the accumulator row of sample t, so
-// all epilogues (ReLU, sigmoid, exp, clamp, loss-side chain rule) are thread-per-sample with no
-// shuffles.  Weight gradients are GEMMs whose reduction dimension is the SAMPLE index; the same
-// shared-memory activation / gradient tiles are re-read MN-major for them (tc05.cuh) and the
-// accumulators stay resident in TMEM across all tiles a persistent CTA processes, then are flushed
-// once with atomics.  Numerics follow torch.autocast(fp16): operands and layer outputs rounded to
+// Mapping: one CTA = one warpgroup of 128 threads = one 128-sample tile = the M dimension of every
+// forward / dgrad GEMM (two m64 halves).  Layer epilogues (ReLU, masks) work on the accumulator
+// fragments directly; the per-sample chain (sigmoid, exp, clamp, loss-side chain rule) runs one
+// sample per thread, its few columns gathered from the fragments by warp shuffles (mlp_common.cuh).
+// Weight gradients are GEMMs whose reduction dimension is the SAMPLE index; the same shared-memory
+// activation / gradient tiles are re-read MN-major for them (wg.cuh) and the accumulators stay
+// resident in registers across all tiles a persistent CTA processes, then are flushed once with
+// atomics.  Numerics follow torch.autocast(fp16): operands and layer outputs rounded to
 // fp16, fp32 accumulation; gradients are carried loss-scaled in fp16 like GradScaler does.
 #include "n2m_common.cuh"
-#include "tc05.cuh"
 #include "mlp_common.cuh"
 #include "../../include/n2m_b200_fused.h"
 
@@ -54,8 +54,7 @@ k_pack_weights(const float* __restrict__ P, uint8_t* __restrict__ wpack) {
 // forward
 // ================================================================================================
 // The specular hidden tile P1 aliases the sigma hidden tile S1, which is dead once sigma_net.1 has completed in round 2 (P1 is written in
-// round 4, S1 again in round 1 of the next tile, after the wait on specular_net.1): 71 KB of shared memory per CTA, i.e. three CTAs per
-// SM (TMEM 3 x 128 columns); measured 34.6 us against 39.5 us for the two-CTA layout with separate tiles (profiles/r2_summary.md).
+// round 4, S1 again in round 1 of the next tile): 71 KB of shared memory per CTA, i.e. three CTAs per SM.
 constexpr uint32_t F_W = 0, F_A = F_W + W_BYTES, F_H = F_A + kTileBytes, F_S1 = F_H + kTileBytes, F_AS2 = F_S1 + 8192, F_BYTES = F_AS2 + 4096;
 
 __global__ void __launch_bounds__(128)
@@ -63,8 +62,7 @@ k_mlp_fwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const int32_t*
           const uint8_t* __restrict__ wpack, float4* __restrict__ out, float* __restrict__ spec_sq_sum,
           uint32_t part, uint32_t nparts) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint64_t bar_mma, bar_tma;
-    __shared__ uint32_t tmem_s;
+    __shared__ uint64_t bar_tma;
     __shared__ float red[4];
     const uint32_t tid = threadIdx.x, warp = tid >> 5;
     // samples [lo, hi) of this part: tiles [t0, t1); the boundary tiles are also computed by the neighbouring parts,
@@ -73,130 +71,49 @@ k_mlp_fwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const int32_t*
     const uint32_t t0 = pr.lo / kTile, t1 = (pr.hi + kTile - 1) / kTile;
     if (pr.hi <= pr.lo || t0 + blockIdx.x >= t1) return;
 
-    if (tid == 0) { tc::mbar_init(&bar_mma, 1); tc::mbar_init(&bar_tma, 1); tc::mbar_init_fence(); }
-    if (warp == 0) tc::tmem_alloc(&tmem_s, 128);
+    if (tid == 0) { wg::mbar_init(&bar_tma, 1); wg::mbar_init_fence(); }
     for (uint32_t i = tid; i < W_BYTES / 16; i += 128)
         reinterpret_cast<uint4*>(smem + F_W)[i] = __ldg(reinterpret_cast<const uint4*>(wpack) + i);
     {   // second K chunk of the specular input tile is always zero
         *reinterpret_cast<uint4*>(smem + F_AS2 + kChunk + tid * 16) = make_uint4(0, 0, 0, 0);
     }
     sync_before_mma();
-    const uint32_t tmem = tmem_s, D0 = tmem, D1 = tmem + 64;
-    const uint32_t lane_t = (warp * 32u) << 16;
-    uint32_t ph_mma = 0, ph_tma = 0;
+    uint32_t ph_tma = 0;
     float spec_sq = 0.f;
-    uint8_t* sW = smem + F_W; uint8_t* sA = smem + F_A; uint8_t* sH = smem + F_H;
-    uint8_t* sS1 = smem + F_S1; uint8_t* sP1 = smem + F_S1; uint8_t* sAs2 = smem + F_AS2;
-    // operand descriptors, built once (only the issuing thread uses them)
-    const tc::OpDesc dA = tc::make_opdesc(opK(sA, 128)), dH = tc::make_opdesc(opK(sH, 128)), dS1 = tc::make_opdesc(opK(sS1, 128)),
-                     dP1 = tc::make_opdesc(opK(sP1, 128)), dAs2 = tc::make_opdesc(opK(sAs2, 128));
-    const tc::OpDesc wC1 = tc::make_opdesc(opK(sW + W_C1, 64)), wC2 = tc::make_opdesc(opK(sW + W_C2, 64)),
-                     wC3 = tc::make_opdesc(opK(sW + W_C3, 16)), wS1 = tc::make_opdesc(opK(sW + W_S1, 32)),
-                     wS2 = tc::make_opdesc(opK(sW + W_S2, 16)), wP1 = tc::make_opdesc(opK(sW + W_P1, 32)),
-                     wP2 = tc::make_opdesc(opK(sW + W_P2, 16));
+    const uint32_t r = sample_row(tid);
 
     for (uint32_t tile = t0 + blockIdx.x; tile < t1; tile += gridDim.x) {
-        if (tid == 0) bulk_g2s(sA, enc_tiles + (size_t)tile * kTileBytes, kTileBytes, &bar_tma);
-        tc::mbar_wait(&bar_tma, ph_tma); ph_tma ^= 1;
-
-        // round 1: first layers of color_net and sigma_net
-        if (tid == 0) {
-            tc::gemm_issue_fast<64, 4, false, false>(D0, dA, wC1, false);
-            tc::gemm_issue_fast<32, 4, false, false>(D1, dA, wS1, false);
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        epi_store_row<64, true>(D0 + lane_t, sH, tid, nullptr);
-        epi_store_row<32, true>(D1 + lane_t, sS1, tid, nullptr);
-        sync_before_mma();
-
-        // round 2: color_net.1, sigma_net.1
-        if (tid == 0) {
-            tc::gemm_issue_fast<64, 4, false, false>(D0, dH, wC2, false);
-            tc::gemm_issue_fast<16, 2, false, false>(D1, dS1, wS2, false);
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        float sigma;
-        {
-            float v[8];
-            tc::tmem_ld8(D1 + lane_t, v);
-            sigma = __expf(round_h(v[0]));                 // trunc_exp forward (activation.py:5-11)
-        }
-        epi_store_row<64, true>(D0 + lane_t, sH, tid, nullptr);       // H2 overwrites H1 (its reader has completed)
-        sync_before_mma();
-
-        // round 3: color_net.2
-        if (tid == 0) {
-            tc::gemm_issue_fast<16, 4, false, false>(D0, dH, wC3, false);
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        float feat[6];
-        {
-            float v[8];
-            tc::tmem_ld8(D0 + lane_t, v);
-#pragma unroll
-            for (int i = 0; i < 6; ++i) feat[i] = sigmoid_h(v[i]);
-        }
-        float cr = feat[0], cg = feat[1], cb = feat[2];
-        float sp[3] = {0.f, 0.f, 0.f};
-        if (p.shading_full) {
-            // specular input [dir(3), feat[3:6]]; dir sits in enc cols 51..53 = chunk 6, elements 3..5
-            const uint4 dq = *reinterpret_cast<const uint4*>(sA + 6 * kChunk + tid * 16);
-            const __half2 d01 = *reinterpret_cast<const __half2*>(&dq.y);     // elements 2,3
-            const __half2 d23 = *reinterpret_cast<const __half2*>(&dq.z);     // elements 4,5
-            const float in[8] = {__high2float(d01), __low2float(d23), __high2float(d23), feat[3], feat[4], feat[5], 0.f, 0.f};
-            store_chunk(sAs2, 0, tid, in);
-            sync_before_mma();
-            if (tid == 0) {
-                tc::gemm_issue_fast<32, 1, false, false>(D1, dAs2, wP1, false);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            epi_store_row<32, true>(D1 + lane_t, sP1, tid, nullptr);
-            sync_before_mma();
-            if (tid == 0) {
-                tc::gemm_issue_fast<16, 2, false, false>(D0, dP1, wP2, false);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            float v[8];
-            tc::tmem_ld8(D0 + lane_t, v);
-#pragma unroll
-            for (int i = 0; i < 3; ++i) sp[i] = sigmoid_h(v[i]);
-            // color = (specular + diffuse).clamp(0, 1) on fp16 tensors (network.py:187)
-            cr = fminf(fmaxf(round_h(sp[0] + cr), 0.f), 1.f);
-            cg = fminf(fmaxf(round_h(sp[1] + cg), 0.f), 1.f);
-            cb = fminf(fmaxf(round_h(sp[2] + cb), 0.f), 1.f);
-        }
-        const uint32_t j = tile * kTile + tid;
+        if (tid == 0) bulk_g2s(smem + F_A, enc_tiles + (size_t)tile * kTileBytes, kTileBytes, &bar_tma);
+        wg::mbar_wait(&bar_tma, ph_tma); ph_tma ^= 1;
+        float sp[3];
+        const float4 o = mlp_fwd_tile(smem + F_A, smem + F_W, smem + F_H, smem + F_S1, smem + F_S1, smem + F_AS2, p.shading_full != 0,
+                                      tid, sp, sync_before_mma);
+        const uint32_t j = tile * kTile + r;
         if (j >= pr.lo && j < pr.hi) {
-            out[j] = make_float4(sigma, cr, cg, cb);
+            out[j] = o;
             spec_sq += sp[0] * sp[0] + sp[1] * sp[1] + sp[2] * sp[2];
         }
-        sync_before_mma();          // all reads of this tile's smem / TMEM are done before the next bulk copy
+        sync_before_mma();          // all reads of this tile's smem are done before the next bulk copy
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) spec_sq += __shfl_xor_sync(0xffffffffu, spec_sq, o);
     if ((tid & 31) == 0) red[warp] = spec_sq;
-    tc::fence_before_sync();
     __syncthreads();
     if (tid == 0 && spec_sq_sum) atomicAdd(spec_sq_sum, red[0] + red[1] + red[2] + red[3]);
-    if (warp == 0) tc::tmem_dealloc(tmem, 128);
 }
 
 // ================================================================================================
 // backward (forward recompute + dgrad + wgrad)
 // ================================================================================================
-__global__ void __launch_bounds__(128)
+// One CTA per SM: 255 registers per thread (-Xptxas -v, CUDA 12.9: 84 B of spills, and ptxas serialises some wgmma issues around
+// register use, C7519).  On an H100 SXM 80 GB at 700 W the kernel takes 0.19 ms of the 1.33 ms lego step (bench.py, stage times).
+__global__ void __launch_bounds__(128, 1)
 k_mlp_bwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const float4* __restrict__ dout,
           const int32_t* __restrict__ counters, const uint8_t* __restrict__ wpack, uint8_t* __restrict__ denc_tiles,
           float* __restrict__ g_mlp, const float* __restrict__ loss_scale, uint32_t part, uint32_t nparts) {
     extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint64_t bar_mma, bar_tma;
-    __shared__ uint32_t tmem_s;
-    const uint32_t tid = threadIdx.x, warp = tid >> 5;
+    __shared__ uint64_t bar_tma;
+    const uint32_t tid = threadIdx.x;
     // rows outside [lo, hi) of a boundary tile belong to a neighbouring part: zero upstream gradient (so they add
     // nothing to the weight gradients; their activations are whatever finite values the tile holds) and no store
     const PartRange pr = part_range(counters, part, nparts);
@@ -204,277 +121,41 @@ k_mlp_bwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const float4* 
     const uint32_t t0 = pr.lo / kTile, t1 = (pr.hi + kTile - 1) / kTile;
     if (pr.hi <= pr.lo || t0 + blockIdx.x >= t1) return;
 
-    if (tid == 0) { tc::mbar_init(&bar_mma, 1); tc::mbar_init(&bar_tma, 1); tc::mbar_init_fence(); }
-    if (warp == 0) tc::tmem_alloc(&tmem_s, 512);
+    if (tid == 0) { wg::mbar_init(&bar_tma, 1); wg::mbar_init_fence(); }
     for (uint32_t i = tid; i < W_BYTES / 16; i += 128)
         reinterpret_cast<uint4*>(smem + B_W)[i] = __ldg(reinterpret_cast<const uint4*>(wpack) + i);
-    uint8_t* sW = smem + B_W; uint8_t* act = smem + B_ACT; uint8_t* grd = smem + B_GRAD;
-    uint8_t* sA = act + A_A; uint8_t* sH2 = act + A_H2; uint8_t* sH1 = act + A_H1; uint8_t* sS1 = act + A_S1;
-    uint8_t* sP1 = act + A_P1; uint8_t* sAs2 = act + A_AS2;
-    uint8_t* sdH = grd + G_DH; uint8_t* sdS1 = grd + G_DS1; uint8_t* sdP1 = grd + G_DP1; uint8_t* sdO = grd + G_DO;
-    uint8_t* sdOs = grd + G_DOS; uint8_t* sdO2 = grd + G_DO2;
-    {   // constant-zero parts of the narrow tiles (their second K chunk, and unused columns of the first)
-        const uint4 z = make_uint4(0, 0, 0, 0);
-        *reinterpret_cast<uint4*>(sAs2 + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdO + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdOs + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdO2 + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sAs2 + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sP1 + tid * 16) = z; *reinterpret_cast<uint4*>(sP1 + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sP1 + 2 * kChunk + tid * 16) = z; *reinterpret_cast<uint4*>(sP1 + 3 * kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdP1 + tid * 16) = z; *reinterpret_cast<uint4*>(sdP1 + kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdP1 + 2 * kChunk + tid * 16) = z; *reinterpret_cast<uint4*>(sdP1 + 3 * kChunk + tid * 16) = z;
-    }
+    zero_narrow_tiles(smem, tid);
     sync_before_mma();
-    const uint32_t tmem = tmem_s;
-    const uint32_t lane_t = (warp * 32u) << 16;
-    const uint32_t K0 = tmem + T_K0, K1 = tmem + T_K1;
-    uint32_t ph_mma = 0, ph_tma = 0;
+    uint32_t ph_tma = 0;
     const bool full = p.shading_full != 0;
     const float ls = loss_scale[0];
     const float spec_reg = (M > 0) ? 2.0f * p.lambda_specular / (float)M * ls : 0.f;   // d/dspec of lambda * mean_j sum_c spec^2
-    bool first = true;                                  // wgrad accumulators are overwritten by the first tile
-
-    const tc::Operand G1 = opMN(sA, 128);               // [A | H2]   as M = 128 input features
-    const tc::Operand G2 = opMN(sH2, 128);              // [H2 | H1]
-    const tc::Operand G3 = opMN(sS1, 128);              // [S1 | P1 | As2 | (don't care)]
+    const uint32_t r = sample_row(tid);
+    WgradAcc wa;
+    wa.zero();
 
     for (uint32_t tile = t0 + blockIdx.x; tile < t1; tile += gridDim.x) {
-        if (tid == 0) bulk_g2s(sA, enc_tiles + (size_t)tile * kTileBytes, kTileBytes, &bar_tma);
-        const uint32_t j = tile * kTile + tid;
+        if (tid == 0) bulk_g2s(smem + B_ACT + A_A, enc_tiles + (size_t)tile * kTileBytes, kTileBytes, &bar_tma);
+        const uint32_t j = tile * kTile + r;
         float4 dv = make_float4(0.f, 0.f, 0.f, 0.f);
         const bool own = j >= pr.lo && j < pr.hi;
         if (own) dv = dout[j];
-        tc::mbar_wait(&bar_tma, ph_tma); ph_tma ^= 1;
-
-        // ---------------- forward recompute ----------------
-        if (tid == 0) {
-            tc::gemm_issue(K0, opK(sA, 128), opK(sW + W_C1, 64), 128, 64, 64, false);
-            tc::gemm_issue(K1, opK(sA, 128), opK(sW + W_S1, 32), 128, 32, 64, false);
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        epi_store_row<64, true>(K0 + lane_t, sH1, tid, nullptr);
-        epi_store_row<32, true>(K1 + lane_t, sS1, tid, nullptr);
-        sync_before_mma();
-        if (tid == 0) {
-            tc::gemm_issue(K0, opK(sH1, 128), opK(sW + W_C2, 64), 128, 64, 64, false);
-            tc::gemm_issue(K1, opK(sS1, 128), opK(sW + W_S2, 16), 128, 16, 32, false);
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        float h_sig;
-        { float v[8]; tc::tmem_ld8(K1 + lane_t, v); h_sig = round_h(v[0]); }
-        epi_store_row<64, true>(K0 + lane_t, sH2, tid, nullptr);
-        sync_before_mma();
-        if (tid == 0) {
-            tc::gemm_issue(K0, opK(sH2, 128), opK(sW + W_C3, 16), 128, 16, 64, false);
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        float feat[6];
-        { float v[8]; tc::tmem_ld8(K0 + lane_t, v);
+        wg::mbar_wait(&bar_tma, ph_tma); ph_tma ^= 1;
+        mlp_bwd_tile(smem, dv, own, full, spec_reg, tid, wa, sync_before_mma, [&](const float (&d)[2][32]) {
+            // the feature gradients -> the tile's rows of the denc tile image (global)
+            uint8_t* img = denc_tiles + (size_t)tile * kTileBytes;
 #pragma unroll
-          for (int i = 0; i < 6; ++i) feat[i] = sigmoid_h(v[i]); }
-        float sp[3] = {0.f, 0.f, 0.f};
-        if (full) {
-            const uint4 dq = *reinterpret_cast<const uint4*>(sA + 6 * kChunk + tid * 16);
-            const __half2 d01 = *reinterpret_cast<const __half2*>(&dq.y);
-            const __half2 d23 = *reinterpret_cast<const __half2*>(&dq.z);
-            const float in[8] = {__high2float(d01), __low2float(d23), __high2float(d23), feat[3], feat[4], feat[5], 0.f, 0.f};
-            store_chunk(sAs2, 0, tid, in);
-            sync_before_mma();
-            if (tid == 0) {
-                tc::gemm_issue(K1, opK(sAs2, 128), opK(sW + W_P1, 32), 128, 32, 16, false);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            epi_store_row<32, true>(K1 + lane_t, sP1, tid, nullptr);
-            sync_before_mma();
-            if (tid == 0) {
-                tc::gemm_issue(K0, opK(sP1, 128), opK(sW + W_P2, 16), 128, 16, 32, false);
-                tc::mma_commit(&bar_mma);
-            }
-            tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-            float v[8];
-            tc::tmem_ld8(K0 + lane_t, v);
+            for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
-            for (int i = 0; i < 3; ++i) sp[i] = sigmoid_h(v[i]);
-        }
-
-        // ---------------- output-side chain rule (thread-per-sample) ----------------
-        float dfeat[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        {
-            const float dcol[3] = {dv.y, dv.z, dv.w};
-            float dO2[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int c = 0; c < 3; ++c) {
-                float g = dcol[c];
-                if (full) {
-                    const float cs = round_h(sp[c] + feat[c]);
-                    if (!(cs >= 0.f && cs <= 1.f)) g = 0.f;            // clamp(0,1) backward
-                    const float dsp = own ? g + spec_reg * sp[c] : 0.f;
-                    dO2[c] = dsp * sp[c] * (1.0f - sp[c]);            // sigmoid backward
+                for (int i = 0; i < 32; i += 2) {
+                    const uint32_t row = frag_row(hh, i, tid), jr = tile * kTile + row;
+                    if (nparts == 1 || (jr >= pr.lo && jr < pr.hi))
+                        *reinterpret_cast<uint32_t*>(img + wg::tile_off(row, frag_col(i, tid), kTile)) = pack2(d[hh][i], d[hh][i + 1]);
                 }
-                dfeat[c] = g;
-            }
-            float dOs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-            dOs[0] = dv.x * __expf(fminf(fmaxf(h_sig, -15.f), 15.f));   // trunc_exp backward (activation.py:13-17)
-            store_chunk(sdOs, 0, tid, dOs);
-            if (full) store_chunk(sdO2, 0, tid, dO2);
-        }
-        sync_before_mma();
-
-        // ---------------- B1: specular_net.1 / sigma_net.1 dgrad + their wgrads ----------------
-        if (tid == 0) {
-            tc::gemm_issue(K0, opK(sdOs, 128), opMN(sW + W_S2, 16), 128, 32, 16, false);            // dS1 (pre-mask)
-            tc::gemm_issue(tmem + T_S2, G3, opMN(sdOs, 128), 128, 16, 128, !first);                  // rows 0..31: S1^T dOs
-            if (full) {
-                tc::gemm_issue(K1, opK(sdO2, 128), opMN(sW + W_P2, 16), 128, 32, 16, false);        // dP1 (pre-mask)
-                tc::gemm_issue(tmem + T_P2, G3, opMN(sdO2, 128), 128, 16, 128, !first);              // rows 32..63: P1^T dO2
-            }
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        epi_store_row<32, false>(K0 + lane_t, sdS1, tid, sS1);
-        if (full) epi_store_row<32, false>(K1 + lane_t, sdP1, tid, sP1);
-        sync_before_mma();
-
-        // ---------------- B2: first-layer dgrads of sigma / specular nets + wgrads ----------------
-        if (tid == 0) {
-            tc::gemm_issue(K0, opK(sdS1, 128), opMN(sW + W_S1, 32), 128, 64, 32, false);            // d enc (sigma part) -> K0
-            tc::gemm_issue(tmem + T_S1, G1, opMN(sdS1, 128), 128, 32, 128, !first);                  // rows 0..63: A^T dS1
-            if (full) {
-                tc::gemm_issue(K1, opK(sdP1, 128), opMN(sW + W_P1, 32), 128, 16, 32, false);        // d As2
-                tc::gemm_issue(tmem + T_P1, G3, opMN(sdP1, 128), 128, 32, 128, !first);              // rows 64..79: As2^T dP1
-            }
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        {
-            if (full) {
-                float v[8];
-                tc::tmem_ld8(K1 + lane_t, v);
-                dfeat[3] = v[3]; dfeat[4] = v[4]; dfeat[5] = v[5];
-            }
-            float dO[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-            for (int i = 0; i < 6; ++i) dO[i] = dfeat[i] * feat[i] * (1.0f - feat[i]);
-            store_chunk(sdO, 0, tid, dO);
-        }
-        sync_before_mma();
-
-        // ---------------- B3: color_net.2 dgrad + wgrad ----------------
-        if (tid == 0) {
-            tc::gemm_issue(K1, opK(sdO, 128), opMN(sW + W_C3, 16), 128, 64, 16, false);             // dH2 (pre-mask)
-            tc::gemm_issue(tmem + T_C3, G2, opMN(sdO, 128), 128, 16, 128, !first);                   // rows 0..63: H2^T dO
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        epi_store_row<64, false>(K1 + lane_t, sdH, tid, sH2);
-        sync_before_mma();
-
-        // ---------------- B4: color_net.1 dgrad + wgrad ----------------
-        if (tid == 0) {
-            tc::gemm_issue(K1, opK(sdH, 128), opMN(sW + W_C2, 64), 128, 64, 64, false);             // dH1 (pre-mask)
-            tc::gemm_issue(tmem + T_C2, G2, opMN(sdH, 128), 128, 64, 128, !first);                   // rows 64..127: H1^T dH2
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        epi_store_row<64, false>(K1 + lane_t, sdH, tid, sH1);
-        sync_before_mma();
-
-        // ---------------- B5: color_net.0 dgrad (accumulated onto the sigma part) + wgrad ----------------
-        if (tid == 0) {
-            tc::gemm_issue(K0, opK(sdH, 128), opMN(sW + W_C1, 64), 128, 64, 64, true);              // d enc += dH1 W_c1
-            tc::gemm_issue(tmem + T_C1, G1, opMN(sdH, 128), 128, 64, 128, !first);                   // rows 0..63: A^T dH1
-            tc::mma_commit(&bar_mma);
-        }
-        tc::mbar_wait(&bar_mma, ph_mma); ph_mma ^= 1; tc::fence_after_sync();
-        {   // this sample's feature gradients -> its row of the denc tile image (global, coalesced per chunk)
-            uint8_t* img = denc_tiles + (size_t)tile * kTileBytes + tid * 16;
-#pragma unroll
-            for (int c0 = 0; c0 < 64; c0 += 16) {
-                float v[16];
-                tc::tmem_ld16(K0 + lane_t + c0, v);
-#pragma unroll
-                for (int q = 0; q < 2; ++q) {
-                    uint4 o;
-                    o.x = pack2(v[8 * q + 0], v[8 * q + 1]); o.y = pack2(v[8 * q + 2], v[8 * q + 3]);
-                    o.z = pack2(v[8 * q + 4], v[8 * q + 5]); o.w = pack2(v[8 * q + 6], v[8 * q + 7]);
-                    if (own || nparts == 1) *reinterpret_cast<uint4*>(img + (c0 / 8 + q) * kChunk) = o;
-                }
-            }
-        }
-        first = false;
+        });
         sync_before_mma();
     }
-
-    // ---------------- flush the weight-gradient accumulators (one row of each per thread) ----------------
-    {
-        const uint32_t i = tid;            // accumulator row = input-feature index within its 128-wide group
-        float v[16];
-        // color_net.0: rows 0..63 = enc column i, cols = out o (64)
-        {
-            const int k = i < 64 ? map_c1(i) : -1;
-#pragma unroll
-            for (int c0 = 0; c0 < 64; c0 += 16) {
-                tc::tmem_ld16(tmem + T_C1 + lane_t + c0, v);
-                if (k >= 0) {
-#pragma unroll
-                    for (int o = 0; o < 16; ++o) atomicAdd(g_mlp + P_C0 + (c0 + o) * 35 + k, v[o]);
-                }
-            }
-        }
-        // color_net.1: rows 64..127 = H1 feature i-64
-#pragma unroll
-        for (int c0 = 0; c0 < 64; c0 += 16) {
-            tc::tmem_ld16(tmem + T_C2 + lane_t + c0, v);
-            if (i >= 64) {
-#pragma unroll
-                for (int o = 0; o < 16; ++o) atomicAdd(g_mlp + P_C1 + (c0 + o) * 64 + (i - 64), v[o]);
-            }
-        }
-        // color_net.2: rows 0..63 = H2 feature i, cols o < 6
-        tc::tmem_ld16(tmem + T_C3 + lane_t, v);
-        if (i < 64) {
-#pragma unroll
-            for (int o = 0; o < 6; ++o) atomicAdd(g_mlp + P_C2 + o * 64 + i, v[o]);
-        }
-        // sigma_net.0: rows 0..63 = enc column i, cols o < 32
-#pragma unroll
-        for (int c0 = 0; c0 < 32; c0 += 16) {
-            tc::tmem_ld16(tmem + T_S1 + lane_t + c0, v);
-            const int k = i < 64 ? map_s1(i) : -1;
-            if (k >= 0) {
-#pragma unroll
-                for (int o = 0; o < 16; ++o) atomicAdd(g_mlp + P_S0 + (c0 + o) * 19 + k, v[o]);
-            }
-        }
-        // sigma_net.1: rows 0..31 = S1 feature i, col 0
-        tc::tmem_ld16(tmem + T_S2 + lane_t, v);
-        if (i < 32) atomicAdd(g_mlp + P_S1 + i, v[0]);
-        if (full) {
-            // specular_net.1: rows 32..63 = P1 feature i-32, cols o < 3
-            tc::tmem_ld16(tmem + T_P2 + lane_t, v);
-            if (i >= 32 && i < 64) {
-#pragma unroll
-                for (int o = 0; o < 3; ++o) atomicAdd(g_mlp + P_P1 + o * 32 + (i - 32), v[o]);
-            }
-            // specular_net.0: rows 64..69 = As2 feature i-64 (< 6), cols o < 32
-#pragma unroll
-            for (int c0 = 0; c0 < 32; c0 += 16) {
-                tc::tmem_ld16(tmem + T_P1 + lane_t + c0, v);
-                if (i >= 64 && i < 70) {
-#pragma unroll
-                    for (int o = 0; o < 16; ++o) atomicAdd(g_mlp + P_P0 + (c0 + o) * 6 + (i - 64), v[o]);
-                }
-            }
-        }
-    }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem, 512);
+    flush_wgrad(wa, g_mlp, full, tid);
 }
 
 
@@ -496,7 +177,7 @@ int n2m_s0_pack_weights(const float* mlp_params, void* wpack, n2m_stream_t strea
 
 static int num_sms() {
     static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
+    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
     return n;
 }
 
@@ -515,7 +196,7 @@ int n2m_s0_mlp_fwd_part(const n2m_s0_params* p, const void* enc_tiles, const int
     N2M_REQUIRE(p && enc_tiles && counters && wpack && out, "s0_mlp_fwd", "null pointer");
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_mlp_fwd", "Mcap must be a positive multiple of 128");
     N2M_REQUIRE(valid_parts(part, nparts), "s0_mlp_fwd", "nparts must be 1, 2, 4 or 8 and part < nparts");
-    const uint32_t grid = min(Mcap / kTile, (uint32_t)(3 * num_sms()));          // 71 KB of shared memory + 128 TMEM columns: 3 CTAs per SM
+    const uint32_t grid = min(Mcap / kTile, (uint32_t)(3 * num_sms()));          // 71 KB of shared memory: 3 CTAs per SM
     k_mlp_fwd<<<grid, 128, F_BYTES, as_stream(stream)>>>(*p, static_cast<const uint8_t*>(enc_tiles), counters,
                                                                 static_cast<const uint8_t*>(wpack), static_cast<float4*>(out), spec_sq_sum,
                                                                 part, nparts);

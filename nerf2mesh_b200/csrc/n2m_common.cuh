@@ -1,4 +1,4 @@
-// n2m_common.cuh -- shared host/device helpers for libn2m_b200 (sm_100a only).
+// n2m_common.cuh -- shared host/device helpers for libn2m_b200 (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>

@@ -39,8 +39,7 @@ __device__ __forceinline__ float adam_update(float p, float g, float& m, float& 
 // Table rows: {density feature fp32 (master lives in the table), 2 colour features (fp32 masters in cmaster,
 // fp16 copy in the table)}.  m/v: [rows] density then [rows][2] colour.  Pure streaming (112 B/row, ~0.7 GB per
 // step): each thread handles kRowsPerThread rows, block-strided so every access stays coalesced, and issues ALL
-// of its loads before the first dependent instruction -- with one row per thread the kernel was latency bound
-// at 1.6 TB/s (profiles/r1_ncu_summary.md).
+// of its loads before the first dependent instruction -- with one row per thread the kernel is latency bound.
 constexpr int kRowsPerThread = 4;
 
 // ZERO = false: the gradient rows are left as they are; the host zeroes that table on a side stream while the NEXT step (which

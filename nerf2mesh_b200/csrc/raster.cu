@@ -1,5 +1,5 @@
-// raster.cu -- stage-1 mesh path (SURVEY.md section 8 a14, BASELINE config 5): triangle rasterization and attribute interpolation as
-// sm_100a kernels, replacing the two nvdiffrast operators the reference calls at nerf/renderer.py:860-863 (`dr.rasterize`,
+// raster.cu -- stage-1 mesh path: triangle rasterization and attribute interpolation as
+// sm_90a kernels, replacing the two nvdiffrast operators the reference calls at nerf/renderer.py:860-863 (`dr.rasterize`,
 // `dr.interpolate`); output convention (u, v, z/w, triangle_id + 1) as consumed at renderer.py:890,894.
 //
 // Design (HBM / L2-atomic bound integer work, no tensor cores): a VISIBILITY BUFFER of one 64-bit word per pixel,
@@ -268,7 +268,7 @@ using namespace n2m;
 
 static int raster_sms() {
     static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 148; }
+    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
     return n;
 }
 

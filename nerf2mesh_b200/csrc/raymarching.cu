@@ -1,4 +1,4 @@
-// raymarching.cu -- occupancy-grid ray marching + volume compositing for sm_100a.
+// raymarching.cu -- occupancy-grid ray marching + volume compositing for sm_90a.
 //
 // Replaces the native layer behind the reference's `raymarching.*` operators
 // (reference: raymarching/src/raymarching.cu).  Arithmetic contract: every value that decides
@@ -12,7 +12,7 @@
 //     regenerates xyz/dir/ts for all samples in parallel, one warp per ray, coalesced;
 //   * the cell test uses only fp32/integer instructions (the reference's double sub-expressions
 //     `0.5 * (..) * H` and `dt * H * 0.5` are exact products of <= 48 significant bits, so a
-//     single fp32 multiply rounds identically -- see DESIGN.md "bit-exact marcher");
+//     single fp32 multiply rounds identically);
 //   * every launch goes to the caller's stream and is checked.
 #include "march_core.cuh"
 

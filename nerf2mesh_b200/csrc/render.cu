@@ -13,7 +13,7 @@
 //   k_r_march     : one thread per alive ray: up to n_step occupied samples from rays_t with the sequential marcher core
 //                   (march_core.cuh; the reference's arithmetic), written as march RECORDS {t, dt, t + dt, ray} in slab order
 //                   i * n_step + k, zero records behind a ray that ran out -- the same record form the training path uses, so
-//   n2m_s0_encode_fwd + n2m_s0_mlp_fwd : the training forward kernels (hash-grid gather into tensor-core tile images, tcgen05 MLPs)
+//   n2m_s0_encode_fwd + n2m_s0_mlp_fwd : the training forward kernels (hash-grid gather into tensor-core tile images, wgmma MLPs)
 //                   evaluate the slab unchanged
 //   k_r_composite : one thread per alive ray: the reference's slab compositor (transmittance carried through weights_sum, stop at
 //                   T < T_thresh or at the zero tail), ray state in the output arrays, survivors appended to the OTHER alive list

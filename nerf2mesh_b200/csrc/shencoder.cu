@@ -1,4 +1,4 @@
-// shencoder.cu -- real spherical-harmonics direction encoding, degree 1..8, for sm_100a.
+// shencoder.cu -- real spherical-harmonics direction encoding, degree 1..8, for sm_90a.
 //
 // Replaces the native layer behind the reference's `sh_encode` / `SHEncoder`
 // (reference: shencoder/src/shencoder.cu:28-439).  The reference spells out 64 polynomials and

@@ -3,7 +3,6 @@
 //   tile images, composite + loss + composite-backward per ray, hash-grid scatter (+TV) backward,
 //   table (de)interleave helpers.  The MLP stages live in mlp_tc.cu, the optimizer in optim.cu.
 #include "march_core.cuh"
-#include "tc05.cuh"
 #include "s0_geom.cuh"
 #include <cstdlib>
 #include "../../include/n2m_b200_fused.h"
@@ -216,8 +215,8 @@ k_s0_records(const int32_t* __restrict__ rays, const float2* __restrict__ tbuf, 
 // POINTS = false: samples come from the march records (training / eval rendering);
 // POINTS = true : explicit positions xyz [P,3] (rays_o) and optional directions [P,3] (rays_d) -- used for the
 //                 density-grid update (renderer.py:1112-1113 evaluates self.density on cell centres), stage 1 and tests.
-// (Evaluating the TV gradient here, where 4 of its 7 stencil values are already in registers, was measured at 194 us against 76 us for
-// this kernel alone plus a 75 us TV launch hidden under the MLP kernels -- profiles/r1_ncu_summary.md -- and was removed.)
+// (The TV gradient is not evaluated here although 4 of its 7 stencil values are in registers: it slows this kernel by more than a
+// separate TV launch costs, and that launch hides under the MLP kernels.)
 template <bool POINTS>
 __device__ __forceinline__ void
 encode_fwd_tile(const n2m_s0_params& p, const float4* __restrict__ recs,
@@ -249,7 +248,7 @@ k_s0_encode_fwd(n2m_s0_params p, const float4* __restrict__ recs, const int32_t*
 // ------------------------------------------------------------------------------------------------
 // encode backward: scatter the (loss-scaled, fp16) feature gradients (template SCATTER) and / or add the TV gradient of the
 // density features (template TV; by default TV is its own launch of this kernel, n2m_s0_tv, see g_tv_mode).
-// L2 atomic throughput bounds this kernel (profiles/r1_ncu_summary.md), so at the coarse levels -- where the
+// L2 atomic throughput bounds this kernel, so at the coarse levels -- where the
 // consecutive samples of a ray (= consecutive lanes) sit in the same lattice cell -- the 8 corner
 // contributions are first summed across each run of same-cell lanes with a segmented warp scan and only the
 // last lane of a run issues the red.global.add.v4.f32.  Fine levels (every lane its own cell) go straight to the atomics.
@@ -377,7 +376,7 @@ encode_bwd_tile(const n2m_s0_params& p, const float4* __restrict__ recs,
 }
 
 // LOOP = false: the grid covers every tile of the slab (whole-batch launch), one tile per block, straight-line code
-// (measured 10 us faster than the looping form); LOOP = true: grid-stride over the part's tiles.
+// (faster than the looping form); LOOP = true: grid-stride over the part's tiles.
 template <bool SCATTER, bool TV, bool LOOP>
 __global__ void __launch_bounds__(kTile)
 k_s0_encode_bwd(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* __restrict__ counters,

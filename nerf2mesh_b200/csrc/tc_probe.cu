@@ -1,8 +1,8 @@
-// tc_probe.cu -- self-test of the tcgen05 primitives in tc05.cuh: one 128 x N x K GEMM with the
+// tc_probe.cu -- self-test of the wgmma primitives in wg.cuh: one 128 x N x K GEMM with the
 // operands in K-major or MN-major form, used by tests/test_gpu_tc05.py to pin the descriptor
 // conventions against torch.matmul before the MLP kernels rely on them.
 #include "n2m_common.cuh"
-#include "tc05.cuh"
+#include "wg.cuh"
 
 namespace n2m {
 namespace {
@@ -10,113 +10,65 @@ namespace {
 // A_phys: [ra x ca] row-major fp16 in global, B_phys: [rb x cb]; D: [128 x N] fp32 row-major.
 //   a_mn == 0: A_phys is [128(M) x K]         a_mn == 1: A_phys is [K x 128(M)]
 //   b_mn == 0: B_phys is [N x K]              b_mn == 1: B_phys is [K x N]
+template <int N, bool A_MN, bool B_MN>
+__device__ __forceinline__ void probe_gemm(const wg::Operand& oa, const wg::Operand& ob, uint32_t K, float* __restrict__ D) {
+    float d[2][N / 2];
+    wg::wgmma_fence();
+    for (uint32_t k = 0; k < K; k += 16) {
+        wg::Mma<N, A_MN, B_MN>::run(d[0], oa.desc(k), ob.desc(k), k > 0);
+        wg::Mma<N, A_MN, B_MN>::run(d[1], oa.shifted(64).desc(k), ob.desc(k), k > 0);
+    }
+    wg::commit(); wg::wait(d);
+    const uint32_t tid = threadIdx.x;
+    for (int h = 0; h < 2; ++h)
+        for (int i = 0; i < N / 2; ++i) {
+            const uint32_t row = 64u * h + 16u * (tid >> 5) + ((tid & 31u) >> 2) + 8u * ((i >> 1) & 1u);
+            const uint32_t col = 8u * (i >> 2) + 2u * (tid & 3u) + (i & 1u);
+            D[row * N + col] = d[h][i];
+        }
+}
+
+template <int N>
+__device__ __forceinline__ void probe_majors(const wg::Operand& oa, const wg::Operand& ob, uint32_t K, float* __restrict__ D) {
+    if (!oa.mn_major && !ob.mn_major) probe_gemm<N, false, false>(oa, ob, K, D);
+    else if (!oa.mn_major) probe_gemm<N, false, true>(oa, ob, K, D);
+    else if (!ob.mn_major) probe_gemm<N, true, false>(oa, ob, K, D);
+    else probe_gemm<N, true, true>(oa, ob, K, D);
+}
+
 __global__ void __launch_bounds__(128)
 k_tc_probe(const __half* __restrict__ A, const __half* __restrict__ B, float* __restrict__ D,
            uint32_t N, uint32_t K, int a_mn, int b_mn) {
     extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ uint64_t bar;
-    __shared__ uint32_t tmem_base_s;
     const uint32_t ra = a_mn ? K : 128u, ca = a_mn ? 128u : K;
     const uint32_t rb = b_mn ? K : N, cb = b_mn ? N : K;
     uint8_t* sa = smem;
     uint8_t* sb = smem + ra * ca * 2;
-    const uint32_t tid = threadIdx.x, warp = tid >> 5;
-
-    if (tid == 0) { tc::mbar_init(&bar, 1); tc::mbar_init_fence(); }
-    if (warp == 0) tc::tmem_alloc(&tmem_base_s, 64);
+    const uint32_t tid = threadIdx.x;
     for (uint32_t i = tid; i < ra * ca; i += 128) {
         const uint32_t r = i / ca, c = i % ca;
-        *reinterpret_cast<__half*>(sa + tc::tile_off(r, c, ra)) = A[i];
+        *reinterpret_cast<__half*>(sa + wg::tile_off(r, c, ra)) = A[i];
     }
     for (uint32_t i = tid; i < rb * cb; i += 128) {
         const uint32_t r = i / cb, c = i % cb;
-        *reinterpret_cast<__half*>(sb + tc::tile_off(r, c, rb)) = B[i];
+        *reinterpret_cast<__half*>(sb + wg::tile_off(r, c, rb)) = B[i];
     }
-    tc::fence_async_smem();
-    tc::fence_before_sync();
+    wg::fence_async_smem();
     __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = tmem_base_s;
-    if (tid == 0) {
-        tc::Operand oa{tc::smem_u32(sa), ra, a_mn != 0};
-        tc::Operand ob{tc::smem_u32(sb), rb, b_mn != 0};
-        tc::gemm_issue(tmem, oa, ob, 128, N, K, false);
-        tc::mma_commit(&bar);
+    const wg::Operand oa{wg::smem_u32(sa), ra, a_mn != 0};
+    const wg::Operand ob{wg::smem_u32(sb), rb, b_mn != 0};
+    switch (N) {
+        case 16: probe_majors<16>(oa, ob, K, D); break;
+        case 32: probe_majors<32>(oa, ob, K, D); break;
+        case 48: probe_majors<48>(oa, ob, K, D); break;
+        case 64: probe_majors<64>(oa, ob, K, D); break;
     }
-    tc::mbar_wait(&bar, 0);
-    tc::fence_after_sync();
-    const uint32_t row = tid;                                  // warp w owns TMEM lanes 32w..32w+31
-    for (uint32_t c0 = 0; c0 < N; c0 += 16) {
-        float v[16];
-        tc::tmem_ld16(tmem + ((warp * 32u) << 16) + c0, v);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) D[row * N + c0 + j] = v[j];
-    }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem, 64);
-}
-
-// micro-benchmark: `reps` GEMMs of 128 x N x K issued back to back by one thread (mode 0: one commit + wait at
-// the end => tensor-pipe throughput; mode 1: commit + wait after every GEMM => issue->completion round trip).
-// out[0] = total cycles (clock64 of the issuing thread), out[1] = MMA instructions issued.
-template <uint32_t N, uint32_t KSTEPS, bool A_MN, bool B_MN>
-__global__ void __launch_bounds__(128)
-k_tc_bench(uint32_t reps, int mode, unsigned long long* __restrict__ out) {
-    extern __shared__ __align__(1024) uint8_t smem[];
-    __shared__ uint64_t bar[2];
-    __shared__ uint32_t tmem_base_s;
-    const uint32_t tid = threadIdx.x, warp = tid >> 5;
-    if (tid == 0) { tc::mbar_init(&bar[0], 1); tc::mbar_init(&bar[1], 1); tc::mbar_init_fence(); }
-    if (warp == 0) tc::tmem_alloc(&tmem_base_s, 128);
-    for (uint32_t i = tid; i < 49152 / 16; i += 128) reinterpret_cast<uint4*>(smem)[i] = make_uint4(0, 0, 0, 0);
-    tc::fence_async_smem(); tc::fence_before_sync();
-    __syncthreads();
-    tc::fence_after_sync();
-    const uint32_t tmem = tmem_base_s;
-    // mode 2: threads 0 and 32 (two warps) issue concurrently into disjoint TMEM columns -- is the 59-cycle
-    // pace per issuing thread or per SM?
-    const bool issuer = tid == 0 || (mode == 2 && tid == 32);
-    if (issuer) {
-        const uint32_t w = tid >> 5;
-        const tc::OpDesc a = tc::make_opdesc(tc::Operand{tc::smem_u32(smem), 128, A_MN});
-        const tc::OpDesc b = tc::make_opdesc(tc::Operand{tc::smem_u32(smem + 32768), B_MN ? 128u : N, B_MN});
-        uint32_t ph = 0;
-        const long long t0 = clock64();
-        for (uint32_t r = 0; r < reps; ++r) {
-            tc::gemm_issue_fast<N, KSTEPS, A_MN, B_MN>(tmem + w * 64, a, b, r > 0);
-            if (mode == 1) { tc::mma_commit(&bar[w]); tc::mbar_wait(&bar[w], ph); ph ^= 1; }
-        }
-        if (mode != 1) { tc::mma_commit(&bar[w]); tc::mbar_wait(&bar[w], ph); }
-        const long long t1 = clock64();
-        out[2 * w] = (unsigned long long)(t1 - t0);
-        out[2 * w + 1] = (unsigned long long)reps * KSTEPS;
-    }
-    tc::fence_before_sync();
-    __syncthreads();
-    if (warp == 0) tc::tmem_dealloc(tmem, 128);
 }
 
 }  // namespace
 }  // namespace n2m
 
 using namespace n2m;
-
-extern "C" int n2m_tc_bench(uint32_t N, uint32_t ksteps, int a_mn, int b_mn, uint32_t reps, int mode, unsigned long long* out,
-                            n2m_stream_t stream) {
-    N2M_REQUIRE(out, "tc_bench", "null pointer");
-    cudaStream_t st = as_stream(stream);
-#define RUN(NN, KS, AM, BM)                                                                                         \
-    if (N == NN && ksteps == KS && (a_mn != 0) == AM && (b_mn != 0) == BM) {                                          \
-        cudaFuncSetAttribute(k_tc_bench<NN, KS, AM, BM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 49152 + 1024);  \
-        k_tc_bench<NN, KS, AM, BM><<<1, 128, 49152 + 1024, st>>>(reps, mode, out);                                    \
-        return check_launch("tc_bench");                                                                             \
-    }
-    RUN(64, 4, false, false) RUN(16, 4, false, false) RUN(64, 4, false, true) RUN(64, 8, true, true) RUN(16, 8, true, true)
-    RUN(32, 8, true, true) RUN(64, 1, false, true) RUN(32, 1, false, true)
-#undef RUN
-    return fail("tc_bench", "configuration not instantiated");
-}
 
 extern "C" int n2m_tc_probe(const void* A, const void* B, float* D, uint32_t N, uint32_t K, int a_mn, int b_mn,
                             n2m_stream_t stream) {

@@ -1,4 +1,4 @@
-"""Drop-in `gridencoder` backed by libn2m_b200.so (sm_100a).
+"""Drop-in `gridencoder` backed by libn2m_b200.so (sm_90a).
 
 Mirrors reference gridencoder/grid.py:24-192: `grid_encode` autograd Function (same positional
 arguments), `GridEncoder` module (same constructor, parameter/buffer names `embeddings`,

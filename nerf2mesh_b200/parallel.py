@@ -1,8 +1,8 @@
 """Multi-GPU data parallelism for the fused stage-0 step: rays are sharded across ranks (one process
 per GPU, each rank draws its own batch), every rank holds a full replica of the tables / MLPs, and the
 only exchange per step is one all-reduce of the flat gradient buffers (hash-table gradients + MLP
-gradients) plus the 4-byte found_inf flag, NCCL over NVLink 5 / NVSwitch.  The reference has no working
-multi-GPU path (its DDP scaffolding is unreachable, SURVEY.md section 2.2)."""
+gradients) plus the 4-byte found_inf flag, NCCL over NVLink / NVSwitch.  The reference has no working
+multi-GPU path (its DDP scaffolding is unreachable)."""
 import torch
 import torch.distributed as dist
 
@@ -246,11 +246,10 @@ class NvlsAdam(PeerAdam):
 
 def make_grad_sync(trainer, mode="auto", group=None):
     """Data-parallel optimizer for `trainer`: 'nvls' (in-switch reduce + multicast all-gather), 'peer' (P2P loads / stores over NVLink),
-    'nccl' (all-reduce + replicated Adam) or 'auto' = the fastest measured for this world size that every rank can set up.
+    'nccl' (all-reduce + replicated Adam) or 'auto' = the one moving the fewest bytes at this world size that every rank can set up.
     Collective: all ranks must call it with the same mode.  Returns (sync, mode_used)."""
-    # measured (profiles/r2_scaling.md): per rank the in-switch reduce-scatter sends 16 B x rows whatever W is, P2P loads
-    # 16 B x rows x (W-1)/W each way, and the multicast all-gather 8 B x rows / W instead of 8 B x rows x (W-1)/W:
-    # peer wins at W = 2 (0.611 vs 0.708 ms/step), NVLS at W = 8 (0.680 vs 0.731); the byte counts cross at W = 4
+    # per rank the in-switch reduce-scatter sends 16 B x rows whatever W is, P2P loads 16 B x rows x (W-1)/W each way, and the
+    # multicast all-gather 8 B x rows / W instead of 8 B x rows x (W-1)/W: the byte counts cross at W = 4
     W = dist.get_world_size(group)
     order = {"auto": ["nvls", "peer", "nccl"] if W > 4 else ["peer", "nccl"], "nvls": ["nvls", "peer", "nccl"],
              "peer": ["peer", "nccl"], "nccl": ["nccl"]}[mode]

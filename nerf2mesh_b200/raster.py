@@ -5,11 +5,11 @@
     out, out_db   = interpolate(attr, rast, tri)                 # attr [1,V,A] -> [1,h,w,A], differentiable w.r.t. attr
     img           = antialias(color, rast, pos, tri, pos_gradient_boost=1.0)   # color [1,h,w,C]; differentiable w.r.t. color and pos
 
-over the sm_100a kernels of csrc/raster.cu and csrc/antialias.cu (C ABI: include/n2m_b200_raster.h).
+over the sm_90a kernels of csrc/raster.cu and csrc/antialias.cu (C ABI: include/n2m_b200_raster.h).
 `rast[..., :] = (u, v, z/w, triangle_id + 1)`.
 Not provided: image-space derivative outputs (`rast_db`, `out_db` are None: the reference ignores them, renderer.py:860-863) and
 gradients of rasterize w.r.t. vertex positions through (u, v) (the reference detaches `xyzs` unless enable_offset_nerf_grad,
-renderer.py:877; the silhouette gradient of `antialias` is the path it relies on) -- see DESIGN.md "stage 1".
+renderer.py:877; the silhouette gradient of `antialias` is the path it relies on).
 No CPU fallback: tensors must live on a CUDA device.
 """
 import torch

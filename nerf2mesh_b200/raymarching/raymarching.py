@@ -1,9 +1,9 @@
-"""Drop-in `raymarching` operators backed by libn2m_b200.so (sm_100a).
+"""Drop-in `raymarching` operators backed by libn2m_b200.so (sm_90a).
 
 Mirrors the reference's Python operator surface (reference: raymarching/raymarching.py:19-386):
 same callable names, argument order, defaults, dtypes, shapes and zero-init contracts, so that
 `nerf/renderer.py` works unmodified (call sites renderer.py:688,711,717,741,776,796,1020,1100,1142).
-Differences that are deliberate and documented in DESIGN.md:
+Deliberate differences:
   * every kernel runs on torch's CURRENT stream (the reference uses the legacy default stream);
   * `march_rays_train` returns ray offsets in ray order (deterministic), the reference's come
     from an atomic counter; per-ray sample sets and counts are bit-identical;

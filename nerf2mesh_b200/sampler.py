@@ -1,7 +1,7 @@
 """Batch sampling on the device: the stage-0 training branch of `NeRFDataset.collate` (nerf/provider.py:300-331) and
 `get_rays` (nerf/utils.py:236-290) for random (image, pixel) pairs, with the pose / image set resident in HBM (the
 reference's `--preload`).  One kernel (`n2m_s0_gen_rays`, include/n2m_b200_fused.h) replaces the ~15 small torch
-kernels and the [H*W] meshgrid the reference builds per step (SURVEY.md section 8f, rank 2)."""
+kernels and the [H*W] meshgrid the reference builds per step."""
 import ctypes
 
 import torch

@@ -1,4 +1,4 @@
-"""Drop-in `shencoder` backed by libn2m_b200.so (sm_100a).
+"""Drop-in `shencoder` backed by libn2m_b200.so (sm_90a).
 
 Mirrors reference shencoder/sphere_harmonics.py:14-89: `sh_encode(inputs, degree,
 calc_grad_inputs)` and the `SHEncoder` module (normalises the direction, degree 1..8)."""

@@ -1,7 +1,7 @@
 """Fused stage-0 train path: host side (allocation, CUDA-graph capture, import/export of
 reference-format parameters).  All arithmetic runs in libn2m_b200.so (include/n2m_b200_fused.h).
 
-`Stage0Trainer` owns the model state in the B200-native layout (interleaved hash tables, packed
+`Stage0Trainer` owns the model state in the library's native layout (interleaved hash tables, packed
 tensor-core weights, flat gradient / Adam buffers) and exposes
 
     loss = trainer.step(rays_o, rays_d, gt, bg_color)        # one full optimizer step
@@ -87,7 +87,7 @@ MLP_LAYOUT = [
 
 
 class Stage0Config:
-    """The operator arguments the reference passes down from `opt` (SURVEY.md section 5 defaults)."""
+    """The operator arguments the reference passes down from `opt`."""
 
     def __init__(self, bound=1.0, contract=False, dt_gamma=0.0, max_steps=1024, grid_size=128, min_near=0.05,
                  T_thresh=1e-4, num_levels=16, base_resolution=16, log2_hashmap_size=19, lambda_mask=0.1,
@@ -159,7 +159,7 @@ class Stage0Trainer:
         self.rows = int(offs[-1])
         R = self.rows
         self.n_mlp = int(_lib.lib.n2m_s0_mlp_param_count())
-        # ---- model state (B200 layout) ----
+        # ---- model state (native layout) ----
         self.table = torch.zeros(R, 2, dtype=torch.float32, device=dev)          # 8-byte entries {f32, half2}
         self.color_master = torch.zeros(R, 2, dtype=torch.float32, device=dev)
         self.gtables = [torch.zeros(R, 4, dtype=torch.float32, device=dev), torch.zeros(R, 4, dtype=torch.float32, device=dev)]
@@ -197,8 +197,10 @@ class Stage0Trainer:
         self.loss_acc = torch.zeros(4, device=dev)          # [0] rgb(+mask) loss, [1] sum |spec|^2
         self.params = S0Params()
         self._fill_params(shading_full=True, gt_has_alpha=True)
-        self.fused_bwd = True               # MLP backward + scatter as one warp-specialised launch (csrc/fused.cu: 201 us against 128 + 174 us
-                                            # for the two stand-alone kernels, profiles/r2_summary.md); False: two launches
+        # True: MLP backward + scatter as one warp-specialised launch (csrc/fused.cu); False: two launches.  The two launches are the
+        # faster choice on the H100 (H100 SXM 80 GB, 700 W: 1.33 against 1.41 ms per lego step in bench.py): the fused kernel's 640
+        # threads leave its MLP warps 96 registers at compile time, beside 120 registers of weight-gradient accumulators.
+        self.fused_bwd = False
         self.fused_fwd = False              # True: gather + MLP forward as one warp-specialised launch (whole batch: needs nparts == 1)
         self.use_cam_near_far = False       # clamp (near, far) with the per-ray values in the slot's cam_nf (--enable_cam_near_far)
         self._tv_overlap = True             # TV gradient as its own launch overlapped with the MLP kernels (tv mode 2)
@@ -526,7 +528,7 @@ class Stage0Trainer:
         * `nparts` > 1: the batch is cut into ray-range parts (include/n2m_b200_fused.h "Ray-range parts"); the chain
           gather -> MLP -> composite -> MLP backward -> scatter of every part runs on its own stream, so the
           latency-bound tensor-core MLP kernels of one part share the SMs with the memory-bound gather / scatter
-          kernels of another (measured in profiles/overlap_probe.py).
+          kernels of another.
         * `tv_overlap`: the TV-gradient kernel (memory bound, independent of the MLPs) runs on a forked stream as well; otherwise it
           is evaluated inside the scatter kernel and only the (normally empty) random-point fallback is launched behind it.
         All forks are joined before returning (and they are graph-capturable: fork/join by events only)."""
@@ -852,9 +854,8 @@ class Stage0Trainer:
         `early_stop` (default): NeRFRenderer.render's inference branch (renderer.py:749-802) with the alive-ray bookkeeping on the device
         (csrc/render.cu): per chunk of `chunk` rays one host call enqueues RENDER_SCHEDULE rounds of march -> gather -> MLPs -> slab
         compositor + survivor compaction; rays stop at T < T_thresh, so samples behind the first surfaces are never evaluated.  One
-        read-back per chunk checks that no ray is left alive (else further rounds run).  Measured on an 800 x 800 view of the analytic
-        scene (profiles/render_probe.py): 10.8 ms per image at chunk = 262 144 (15.3 ms at 65 536) against 33.4 ms for the all-samples
-        path, same image to 9e-5.  `render_rounds` / `render_rows` afterwards: rounds of the last chunk, sample rows evaluated in total.
+        read-back per chunk checks that no ray is left alive (else further rounds run); bench.py's `psnr.eval_render` times it
+        against the all-samples path on an 800 x 800 view.  `render_rounds` / `render_rows` afterwards: rounds of the last chunk, sample rows evaluated in total.
         `early_stop=False`: every ray's samples are marched up front and evaluated with the training kernels in chunks of `num_rays`
         (the compositor stops at T_thresh, the gather / MLP work behind it is spent)."""
         self.drop_prefetch()

@@ -11,7 +11,7 @@ the model state (hash tables, MLP weights, optimizer moments, GradScaler state) 
 image-loss gradient w.r.t. the vertices in `vertex_gradient()` -- the quantity the reference's vertex optimizer consumes.
 `lr_vert > 0` also trains the vertex offsets as the reference's default stage 1 does (`vertices_offsets`, renderer.py:160,180: an Adam
 group with lr_vert; regularisers lambda_lap * laplacian_smooth_loss (uniform) + lambda_offsets * mean(sum(offsets^2)), utils.py:750-779).
-Not built (DESIGN.md "stage 1"): re-meshing (`refine_and_decimate`, CPU mesh libraries) and the pytorch3d regularisers that are off by
+Not built: re-meshing (`refine_and_decimate`, CPU mesh libraries) and the pytorch3d regularisers that are off by
 default (lambda_normal, lambda_edgelen).
 """
 import ctypes
@@ -140,7 +140,7 @@ class Stage1Trainer:
         """One optimizer step on one view: mvp [4,4], rays_d [h0*w0,3] (unnormalised), gt [h0*w0, 3 or 4], bg [h0*w0,3].
         `use_graph`: the step is captured once per view (keyed by the addresses of its device-resident tensors, which must then stay
         valid and in place -- the dataset of a stage-1 run is a fixed set of views) and replayed as one CUDA graph: ~17 launches and a
-        handful of torch ops leave the host's critical path (the eager step is host-bound at this size, profiles/r2_summary.md)."""
+        handful of torch ops leave the host's critical path (the eager step is host-bound at this size)."""
         t0 = self.t0
         if lr is not None:
             t0.opt_state[4:5].fill_(float(lr))

@@ -3,7 +3,7 @@ are available): Lego-like orbit cameras, ray sampling exactly as the reference's
 an analytic "bricks" scene (axis-aligned coloured boxes) with its occupancy grid in the
 reference's Morton/bitfield layout, and analytic ground-truth colours for those rays.
 
-Shapes / conventions follow SURVEY.md section 8(d): 100 poses on the upper hemisphere at radius
+Shapes / conventions: 100 poses on the upper hemisphere at radius
 4.031 * 0.8, 800x800, fl = 400 / tan(0.5 * 0.6911), rays exactly as nerf/utils.py:282-290
 (unnormalised directions, -z forward, y flipped), pixel ids via randint as provider.py:303 and
 utils.py:271.  Pure torch/numpy host code; no kernels.
@@ -79,7 +79,7 @@ def make_bricks(n_boxes=40, extent=0.7, seed=1, min_size=0.08, max_size=0.25):
 
 
 def make_garden_bricks(seed=1):
-    """Garden-like content for the bound-16 / 5-cascade configuration (SURVEY.md section 8d config 4): the central object of
+    """Garden-like content for the bound-16 / 5-cascade configuration: the central object of
     make_bricks(), a ground slab through the scene and a sparse shell of far boxes, so that samples fall inside AND outside the unit
     cube and in every cascade."""
     lo, hi, rgb = make_bricks(seed=seed)
@@ -183,7 +183,7 @@ def occupancy_regime(regime, H=128, cascades=1, bound=1.0, seed=1):
     return grid, packbits_host(grid), bricks
 
 
-# ---- synthetic closed meshes and projections for stage 1 (SURVEY.md section 8d config 5: icosphere-like, F up to 3e5) ----
+# ---- synthetic closed meshes and projections for stage 1 ----
 def icosphere(subdiv=3, radius=0.6):
     t = (1.0 + 5 ** 0.5) / 2
     v = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],

@@ -1,9 +1,9 @@
 """Train the fused stage-0 pipeline on the analytic bricks scene with the reference's lego recipe and report
-test PSNR (there are no datasets in this environment; SURVEY.md section 8d):
+test PSNR (no dataset is needed):
 
     python -m nerf2mesh_b200.train_synthetic --iters 3000
 
-Recipe (reference defaults, SURVEY.md section 5): 4096 rays/step, lr 1e-2 with LambdaLR warm-up 500 it then
+Recipe (reference defaults): 4096 rays/step, lr 1e-2 with LambdaLR warm-up 500 it then
 0.1^((it-500)/(iters-500)) (main.py:239), 'diffuse' shading for the first 1000 steps (utils.py:669-672), density
 grid update every 16 steps (utils.py:1155-1156), random background (utils.py:660), lambda_tv 1e-8 (readme.md:64).
 """

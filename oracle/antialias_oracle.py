@@ -3,7 +3,7 @@
 CPU (numpy, float64, plain loops) restatement of the third nvdiffrast operator of the reference's stage 1, `dr.antialias`
 (call sites nerf/renderer.py:886-887: `dr.antialias(alphas | rgbs, rast, vertices_clip, self.triangles, pos_gradient_boost=...)`,
 the only differentiable path from the image loss to `vertices_offsets` when `enable_offset_nerf_grad` is off).  nvdiffrast is not
-vendored under /root/reference, not installed here, and the reference pins no version, so the library cannot be run: this file
+vendored in the reference tree, not installed here, and the reference pins no version, so the library cannot be run: this file
 restates the PUBLISHED algorithm (Laine et al., "Modular Primitives for High-Performance Differentiable Rendering", section 3.4
 "Antialiasing"; nvdiffrast documentation, "antialias") and is anchored on the reference's call sites and on hand-computable
 cases (tests/test_antialias_oracle.py).  The reference's tests hold no vectors at this boundary: PARITY UNPINNED.

@@ -2,7 +2,7 @@
 
 CPU (numpy, float64, plain loops over the active cells) marching cubes with the conventions of csrc/mcubes.cu, the checker of those
 kernels.  The reference calls the third-party PyMCubes (`mcubes.marching_cubes`, nerf/renderer.py:526-529), which is neither vendored
-under /root/reference nor installed here, and pins no version: its output cannot be produced, and the classic 256-case table it ships
+in the reference tree nor installed here, and pins no version: its output cannot be produced, and the classic 256-case table it ships
 is not transcribed here -- the case table is GENERATED (nerf2mesh_b200/mc_table.py: crossing points traced around the cube's faces,
 inside corners cut off separately on ambiguous faces).  What is shared with the library by construction: vertices lie on the grid edges
 at the linear-interpolation crossing, in index coordinates, shared between cells.  What may differ: the triangulation inside a cell, the

@@ -3,7 +3,7 @@
 CPU (numpy, float64) restatement of the two nvdiffrast operators the reference's stage 1 calls
 (`dr.rasterize`, `dr.interpolate`; call sites nerf/renderer.py:860-863, consumers :890 `rast[..., 2]` as depth and :894
 `rast[..., -1] - 1` as triangle id).  nvdiffrast is a third-party dependency of the reference that is NOT vendored under
-/root/reference and not installed in this image; the reference pins no version (readme.md:28-29 installs the git head).  Its published
+the reference tree and not installed in this image; the reference pins no version (readme.md:28-29 installs the git head).  Its published
 output convention (nvdiffrast documentation, "rasterize" / "interpolate"):
 
     rast[n, y, x] = (u, v, z/w, triangle_id + 1), all zero where no triangle covers the pixel centre;

@@ -3,8 +3,8 @@
 CPU restatement (numpy, float32) of the reference's ray-marching / compositing kernels,
 vectorised over rays.  Each function cites the reference lines it follows.
 
-Pinning: the reference has no tests or golden vectors (SURVEY.md section 4); this oracle is
-pinned against outputs of the reference's own CUDA kernels (oracle/_ref, run on a B200) stored
+Pinning: the reference has no tests or golden vectors; this oracle is
+pinned against outputs of the reference's own CUDA kernels (oracle/_ref) stored
 under tests/golden/ (see tests/golden/make_golden.py and tests/test_oracle_golden.py).
 Arithmetic notes: the reference is built with -use_fast_math, i.e. FMA contraction, approximate
 reciprocal and ex2, flush-to-zero.  numpy cannot reproduce MUFU.RCP / MUFU.EX2 bit-for-bit, so this

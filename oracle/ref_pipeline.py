@@ -1,8 +1,8 @@
 """oracle/ref_pipeline.py -- TEST / BASELINE INFRASTRUCTURE, NOT PRODUCT.
 
 The reference's stage-0 training pipeline re-composed around the reference's OWN, unmodified CUDA kernels
-(oracle/_ref: raymarching / gridencoder extensions compiled from /root/reference by oracle/build_ref.py).
-It exists so that the same B200 can run "the reference" beside nerf2mesh_b200:
+(oracle/_ref: raymarching / gridencoder extensions compiled from the reference tree by oracle/build_ref.py).
+It exists so that the same GPU can run "the reference" beside nerf2mesh_b200:
 
   * same-box throughput baseline (samples/s of the reference CUDA path), and
   * PSNR-vs-reference on the synthetic scene (BASELINE.json: "PSNR vs ref").

@@ -1,7 +1,7 @@
 """oracle/torch_ema_port.py -- TEST INFRASTRUCTURE, NOT PRODUCT.
 
 Restatement of `torch_ema.ExponentialMovingAverage` (third-party dependency of the reference, imported at nerf/utils.py:29, NOT
-vendored under /root/reference and not installed in this image; the reference pins no version -- requirements.txt lists
+vendored in the reference tree and not installed in this image; the reference pins no version -- requirements.txt lists
 `torch-ema` bare).  Published algorithm (torch_ema/ema.py of the 0.3 release, the current one when the reference was written):
 
     __init__(parameters, decay, use_num_updates=True): shadow_params = [p.clone().detach() for p in parameters]; num_updates = 0

@@ -6,7 +6,7 @@ PyTorch (CPU) restatement of one stage-0 train step of the reference:
   +  post_train_step TV gradient (utils.py:801-823)  +  Adam(eps=1e-15) (main.py:221).
 The reference has no CPU path (every operator calls .cuda()); this module composes the oracle's
 numpy marcher, a differentiable torch hash-grid lookup and a padded differentiable compositor,
-which is what BASELINE.md calls "the repo's own PyTorch restatement".
+the repo's own PyTorch restatement of the reference step.
 
 `amp=True` emulates torch.autocast(fp16) + the reference's fp16 colour table: Linear inputs,
 weights and outputs are rounded to fp16 (fp32 accumulate), sigmoid/clamp run on fp16 values.
@@ -108,7 +108,7 @@ class _TruncExp(torch.autograd.Function):
 
 
 class OracleField(nn.Module):
-    """Parameter names match the reference checkpoint schema (SURVEY.md section 5):
+    """Parameter names match the reference checkpoint schema:
     encoder.embeddings, encoder_color.embeddings, sigma_net.net.{0,1}.weight,
     color_net.net.{0,1,2}.weight, specular_net.net.{0,1}.weight."""
 

@@ -1,5 +1,4 @@
-"""ctypes binding of libn2m_probes.so: the tcgen05 layout probe / issue-rate benchmark (csrc/tc_probe.cu) and the spread-RED
-benchmark (csrc/red_probe.cu).  Test and profiling infrastructure -- not part of the product library libn2m_b200.so."""
+"""ctypes binding of libn2m_probes.so: the wgmma layout probe (csrc/tc_probe.cu).  Test and profiling infrastructure -- not part of the product library libn2m_b200.so."""
 import ctypes
 import os
 
@@ -8,8 +7,7 @@ from nerf2mesh_b200._lib import I, P, U, check
 
 PATH = os.path.join(os.path.dirname(os.path.abspath(_lib.__file__)), "libn2m_probes.so")
 lib = ctypes.CDLL(PATH, mode=ctypes.RTLD_GLOBAL)
-for _n, _a in {"n2m_tc_probe": [P, P, P, U, U, I, I, P], "n2m_tc_bench": [U, U, I, I, U, I, P, P],
-               "n2m_red_bench": [I, P, U, U, U, U, P]}.items():
+for _n, _a in {"n2m_tc_probe": [P, P, P, U, U, I, I, P]}.items():
     _f = getattr(lib, _n); _f.argtypes = _a; _f.restype = ctypes.c_int
 
 

@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -27,19 +27,27 @@ def pytest_collection_modifyitems(config, items):
             item.add_marker(skip)
 
 
-@pytest.fixture(scope="session")
-def ref_raymarching():
-    from oracle.build_ref import load_ref
-    return load_ref("_ref_raymarching")
+def _reference(request, name):
+    # the reference's kernels, or their recorded outputs (tests/refreplay.py)
+    import refreplay
+    from oracle.build_ref import built, load_ref
+    mod = load_ref("_ref_" + name) if (refreplay.RECORD or built("_ref_" + name)) else None
+    if refreplay.RECORD:
+        request.addfinalizer(refreplay.save_all)
+    # recordings are keyed by test file name and test name (with parameters): independent of the directory pytest runs from
+    return refreplay.Replay(name, mod, f"{os.path.basename(str(request.node.fspath))}::{request.node.name}")
 
 
-@pytest.fixture(scope="session")
-def ref_gridencoder():
-    from oracle.build_ref import load_ref
-    return load_ref("_ref_gridencoder")
+@pytest.fixture
+def ref_raymarching(request):
+    return _reference(request, "raymarching")
 
 
-@pytest.fixture(scope="session")
-def ref_shencoder():
-    from oracle.build_ref import load_ref
-    return load_ref("_ref_shencoder")
+@pytest.fixture
+def ref_gridencoder(request):
+    return _reference(request, "gridencoder")
+
+
+@pytest.fixture
+def ref_shencoder(request):
+    return _reference(request, "shencoder")

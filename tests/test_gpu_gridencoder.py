@@ -8,6 +8,7 @@ import torch
 
 import cases
 import refcall
+import refreplay
 from nerf2mesh_b200._lib import call, ptr, stream
 from nerf2mesh_b200.gridencoder import GridEncoder, grid_encode
 from oracle import grid_oracle
@@ -44,10 +45,14 @@ def test_forward_bit_exact(ref_gridencoder, name, partial):
     inputs, emb, offsets = c["inputs"].cuda(), c["embeddings"].cuda(), c["offsets"].cuda()
     L = c["L"]
     max_level = L // 2 if partial else L
-    o0, dy0 = refcall.grid_fwd(ref_gridencoder, inputs, emb, offsets, c["S"], c["H"], max_level, c["gridtype"], c["align"], c["interp"], True)
+
+    def summary(mod):        # the reference's outputs as digests (bit-exact comparison)
+        o0, dy0 = refcall.grid_fwd(mod, inputs, emb, offsets, c["S"], c["H"], max_level, c["gridtype"], c["align"], c["interp"], True)
+        return {"o": refreplay.digest(o0), "dy": refreplay.digest(dy0)}
+    ref = ref_gridencoder.summary(summary)
     o1, dy1 = ours_fwd(inputs, emb, offsets, c["S"], c["H"], max_level, c["gridtype"], c["align"], c["interp"], True)
-    assert torch.equal(o0, o1), f"outputs differ: {(o0.float() - o1.float()).abs().max()}"
-    assert torch.equal(dy0, dy1), f"dy_dx differ: {(dy0.float() - dy1.float()).abs().max()}"
+    assert refreplay.digest(o1) == ref["o"], "outputs differ"
+    assert refreplay.digest(dy1) == ref["dy"], "dy_dx differ"
     assert o1.abs().max() > 0
 
 

@@ -233,7 +233,7 @@ def test_fused_backward_equals_two_kernel_backward(shading, n_rays, nparts):
         res.append({k: v.clone() for k, v in tr.export_reference_grads().items()})
         assert tr.opt_state[3].item() == 0
     M = int(tr.counters[1].item())
-    assert M > 128 * (148 if n_rays > 1000 else 1)
+    assert M > 128 * (torch.cuda.get_device_properties(0).multi_processor_count if n_rays > 1000 else 1)
     for name in res[0]:
         a, r = res[1][name].double(), res[0][name].double()
         assert r.abs().max().item() > 0 or (shading == "diffuse" and name.startswith("specular")), name
@@ -395,7 +395,7 @@ def _operator_march(tr, Nr):
 
 @pytest.mark.parametrize("name,lambda_entropy", [("lego_converged", 1e-2), ("garden_cascades", 1e-3)])
 def test_entropy_and_cascades_through_the_fused_step(name, lambda_entropy):
-    """The garden recipe's extras through the fused path (scripts/runall_360_outdoor.sh, SURVEY.md section 8d config 4):
+    """The garden recipe's extras through the fused path (scripts/runall_360_outdoor.sh of the reference):
     bound 16 => 5 cascades and a 32768-resolution grid, dt_gamma 1/256, entropy regulariser on weights and weights_sum
     (utils.py:728-733, with the reference's grad_weights folding, raymarching.cu:676), TV weight x10 outside the unit cube
     (utils.py:815-821).  Samples are taken from the operator-level marcher (asserted identical to the fused one), everything
@@ -511,13 +511,28 @@ def test_tv_random_point_fallback(ref_gridencoder):
     ours = tr.export_reference_grads()["encoder.embeddings"]
     st = tr.export_reference_state()
     emb = st["encoder.embeddings"].contiguous()
-    grad = torch.zeros_like(emb)
     S_ = float(np.log2(tr.cfg.per_level_scale))
-    ref_gridencoder.grad_total_variation(pts, emb, grad, tr.offsets, tr.cfg.lambda_tv, pts.shape[0], 3, 1, 16, S_, 16, 0, False)
-    torch.cuda.synchronize()
-    scale = grad.abs().max().item()
+
+    def summary(mod):
+        # the reference's gradient table is 24 MB: its exact scale and number of non-zero entries, and a fixed, seeded sample of
+        # 32768 of its non-zero entries plus 8192 entries drawn from the whole table
+        grad = torch.zeros_like(emb)
+        mod.grad_total_variation(pts, emb, grad, tr.offsets, tr.cfg.lambda_tv, pts.shape[0], 3, 1, 16, S_, 16, 0, False)
+        torch.cuda.synchronize()
+        flat = grad.reshape(-1)
+        nz = flat.nonzero().flatten().cpu()
+        g = torch.Generator().manual_seed(0)
+        idx = torch.cat([nz[torch.randperm(nz.numel(), generator=g)[:32768]],
+                         torch.randint(0, flat.numel(), (8192,), generator=g)]).unique()
+        return {"scale": np.array(flat.abs().max().item()), "nnz": np.array(nz.numel()), "idx": idx.int().numpy(),
+                "val": flat[idx.cuda()].cpu().numpy()}
+    ref = ref_gridencoder.summary(summary)
+    scale = float(ref["scale"])
     assert scale > 0
-    assert (ours - grad).abs().max().item() <= 1e-4 * scale, ((ours - grad).abs().max().item(), scale)
+    o = ours.reshape(-1)
+    assert abs(int((o != 0).sum().item()) - int(ref["nnz"])) <= 1e-3 * int(ref["nnz"]), (int((o != 0).sum().item()), int(ref["nnz"]))
+    err = (o[torch.from_numpy(ref["idx"]).long().cuda()] - torch.from_numpy(ref["val"]).cuda()).abs().max().item()
+    assert err <= 1e-4 * scale, (err, scale)
     # a new point set every optimizer step
     pts2 = torch.zeros_like(pts)
     tr.opt_state[2] += 1
@@ -538,7 +553,7 @@ def test_tv_random_point_fallback(ref_gridencoder):
 
 @pytest.mark.parametrize("shading,n_rays", [("full", 96), ("diffuse", 96), ("full", 4096)])
 def test_fused_forward_equals_two_kernel_forward(shading, n_rays):
-    """k_s0_fwd_fused (gather groups -> shared-memory tile image -> tcgen05 MLP rounds, TMA store of the image for the backward) vs
+    """k_s0_fwd_fused (gather groups -> shared-memory tile image -> wgmma MLP rounds, TMA store of the image for the backward) vs
     k_s0_encode_fwd followed by k_mlp_fwd: bit-identical tile images and outputs (same per-sample arithmetic); 4096 rays give every CTA
     several tiles per gather group (buffer reuse, both barrier phases, the bulk-store read fence)."""
     tr, b = make(shading, N=n_rays)

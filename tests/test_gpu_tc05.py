@@ -1,5 +1,5 @@
-"""Pins the tcgen05 descriptor conventions of csrc/tc05.cuh against torch.matmul: one
-128 x N x K UMMA with each operand K-major or MN-major (all four combinations the fused MLP
+"""Pins the wgmma descriptor conventions of csrc/wg.cuh against torch.matmul: one
+128 x N x K GEMM (two m64 wgmma halves) with each operand K-major or MN-major (all four combinations the fused MLP
 kernels use: forward, dgrad, wgrad)."""
 import pytest
 import torch

@@ -4,7 +4,8 @@
 // gridencoder.cu:248-339) in ONE persistent kernel.  The stand-alone kernels (k_mlp_bwd: a latency-bound chain of ten dependent
 // tensor-core rounds per tile, low occupancy; k_s0_encode_bwd: bound by the rate of spread red.global.add.v4.f32, no tensor or
 // shared-memory use) leave each other's resources idle and run back to back.  Here one CTA per SM holds
-//     warps 0-3  : the MLP backward of k_mlp_bwd, one 128-sample tile at a time (one warpgroup issuing the wgmma rounds);
+//     warps 0-3  : the MLP backward, one 128-sample tile at a time: one warpgroup runs the chain of k_mlp_bwd and issues each
+//                  weight-gradient step itself as soon as the chain has published its tiles (mlp_common.cuh, InlineWgrad);
 //                  the feature gradients of a finished tile go to a double-buffered shared-memory image instead of HBM,
 //     warps 4-19 : the scatter of the previous tile: warp = (32-sample group, level l mod 4), lane = sample, so consecutive lanes
 //                  are consecutive samples of a ray and runs of same-cell lanes are merged before the RED as before (the scatter is
@@ -24,14 +25,16 @@ constexpr uint32_t kMlpThreads = 128, kScatWarps = 16, kFusedThreads = kMlpThrea
 // register budget (setmaxnreg, multiples of 8).  The kernel starts with 96 registers per thread; setmaxnreg.inc can only take what
 // setmaxnreg.dec of the other warps returned to the CTA pool: 512 x (96 - 72) = 12 288 >= 128 x (184 - 96) = 11 264.
 // ptxas (CUDA 12.9, sm_90a) compiles this 640-thread kernel at 96 registers per thread whatever these budgets say, and the MLP
-// warps' wgmma accumulators (120 weight-gradient registers beside a layer's 64) spill: 960 B of stack, about 1.5 KB of spill
-// stores per thread (-Xptxas -v).  That is why the two-launch backward (k_mlp_bwd + k_s0_encode_bwd) is the default (stage0.py).
+// warps' wgmma accumulators (120 weight-gradient registers beside a layer's 64) spill: 656 B of stack, 1,168 B of spill stores
+// and 1,124 B of spill loads per thread, and one C7512 advisory (wgmma serialised for lack of registers; -Xptxas -v).  On an
+// H100 80GB HBM3 at 700 W it takes 0.67 ms of a 1.33 ms lego step, where the two-launch backward (k_mlp_bwd + k_s0_encode_bwd)
+// gives a 1.27 ms step; the two launches are therefore the default (stage0.py).
 constexpr uint32_t kMlpRegs = 184, kScatRegs = 72;
 static_assert(kScatWarps * 32 * (96 - kScatRegs) >= kMlpThreads * (kMlpRegs - 96), "setmaxnreg.inc must fit in what setmaxnreg.dec releases");
 constexpr uint32_t D_CHUNKS = 7;                          // gradient columns 0..55 (cols 3..50 are used)
 constexpr uint32_t D_BYTES = D_CHUNKS * kChunk;           // 14336
-constexpr uint32_t FB_DENC = B_BYTES;
-constexpr uint32_t FB_BYTES = B_BYTES + 2 * D_BYTES;      // 168960
+constexpr uint32_t FB_DENC = B_SET + T_BYTES;             // weights + one tile set
+constexpr uint32_t FB_BYTES = FB_DENC + 2 * D_BYTES;      // 152576
 
 __device__ __forceinline__ void bar_mlp() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
 // MLP warps only: make generic smem writes visible to the tensor core, meet at named barrier 1
@@ -155,9 +158,10 @@ k_s0_bwd_fused(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const flo
     if (tid >= kMlpThreads && tid < kMlpThreads + kLevels) s_lc[tid - kMlpThreads] = make_level_const(offsets, tid - kMlpThreads, p.S, p.base_res);
     for (uint32_t i = tid; i < W_BYTES / 16; i += kFusedThreads)
         reinterpret_cast<uint4*>(smem + B_W)[i] = __ldg(reinterpret_cast<const uint4*>(wpack) + i);
-    uint8_t* sA = smem + B_ACT + A_A;
+    uint8_t* set = smem + B_SET;
+    uint8_t* sA = set + T_A;
     uint8_t* sD = smem + FB_DENC;
-    if (tid < kMlpThreads) zero_narrow_tiles(smem, tid);
+    if (tid < kMlpThreads) zero_narrow_tiles(set, tid);
     wg::fence_async_smem();
     __syncthreads();
 
@@ -227,7 +231,8 @@ k_s0_bwd_fused(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const flo
             const bool own = j >= pr.lo && j < pr.hi;
             if (own) dv = dout[j];
             wg::mbar_wait(&bar_tma, ph_tma); ph_tma ^= 1;
-            mlp_bwd_tile(smem, dv, own, full, spec_reg, tid, wa, sync_mlp, [&](const float (&d)[2][32]) {
+            InlineWgrad<void (*)()> wgrad{set, wa, sync_mlp};     // the chain and the weight-gradient steps on this one warpgroup
+            mlp_bwd_chain(smem + B_W, set, dv, own, full, spec_reg, tid, sync_mlp, wgrad, [&](const float (&d)[2][32]) {
                 // the scatter warps must have taken the buffer's previous contents (two tiles ago) before it is overwritten
                 wg::mbar_wait(&bar_empty[buf], (use & 1) ^ 1);
                 // the feature gradients -> the shared-memory gradient image (zeros for rows of other parts)

@@ -82,57 +82,70 @@ __device__ __forceinline__ void row_cols(const float (&acc)[2][N / 2], float (&v
 // 128 x NCOL accumulator -> optional ReLU / mask -> fp16 128-row chunk-major tile.  mask_tile != nullptr: zero where the fp16
 // activation stored there is <= 0.  ReLU and the mask are applied on packed half2 values, bit-identical to the fp32 formulation
 // (rounding to fp16 commutes with max(., 0) and with zeroing).
+// Shared-memory accesses by 32-bit shared-window address: one base register per tile and immediate offsets, where generic
+// pointers would take a 64-bit address register pair per access of an unrolled epilogue.
+__device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" :: "r"(addr), "r"(v) : "memory"); }
+__device__ __forceinline__ uint32_t lds32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
+__device__ __forceinline__ __half2 bits_h2(uint32_t u) { return *reinterpret_cast<__half2*>(&u); }
+
 template <int NCOL, bool RELU>
 __device__ __forceinline__ void epi_store(const float (&acc)[2][NCOL / 2], uint8_t* tile, uint32_t tid, const uint8_t* mask_tile) {
     const __half2 zero2 = __float2half2_rn(0.f);
+    const uint32_t t = wg::smem_u32(tile) + wg::tile_off(frag_row(0, 0, tid), frag_col(0, tid), kTile);
+    const uint32_t m = mask_tile ? wg::smem_u32(mask_tile) + wg::tile_off(frag_row(0, 0, tid), frag_col(0, tid), kTile) : 0u;
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh)
 #pragma unroll
         for (int i = 0; i < NCOL / 2; i += 2) {
-            const uint32_t off = wg::tile_off(frag_row(hh, i, tid), frag_col(i, tid), kTile);
+            // offset of this fragment pair from the thread's first one: a compile-time constant
+            const uint32_t off = wg::tile_off(64u * hh + 8u * ((i >> 1) & 1), 8u * (i >> 2), kTile);
             __half2 h = __floats2half2_rn(acc[hh][i], acc[hh][i + 1]);
             if (RELU) h = __hmax2(h, zero2);
-            if (mask_tile) h = __hmul2(h, __hgt2(*reinterpret_cast<const __half2*>(mask_tile + off), zero2));
-            *reinterpret_cast<__half2*>(tile + off) = h;
+            if (mask_tile) h = __hmul2(h, __hgt2(bits_h2(lds32(m + off)), zero2));
+            sts32(t + off, h2_bits(h));
         }
 }
 
 __device__ __forceinline__ void store_chunk(uint8_t* tile, uint32_t chunk, uint32_t r, const float (&v)[8]) {
-    uint4 o;
-    o.x = pack2(v[0], v[1]); o.y = pack2(v[2], v[3]); o.z = pack2(v[4], v[5]); o.w = pack2(v[6], v[7]);
-    *reinterpret_cast<uint4*>(tile + chunk * kChunk + r * 16) = o;
+    const uint32_t a = wg::smem_u32(tile) + chunk * kChunk + r * 16;
+    asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};"
+                 :: "r"(a), "r"(pack2(v[0], v[1])), "r"(pack2(v[2], v[3])), "r"(pack2(v[4], v[5])), "r"(pack2(v[6], v[7])) : "memory");
 }
 
 __device__ __forceinline__ wg::Operand opK(const uint8_t* tile, uint32_t rows) { return wg::Operand{wg::smem_u32(tile), rows, false}; }
 __device__ __forceinline__ wg::Operand opMN(const uint8_t* tile, uint32_t rows) { return wg::Operand{wg::smem_u32(tile), rows, true}; }
 
+// ---- backward shared memory: the packed weights, then one or more tile sets (one per 128-sample tile in flight) --------------
+// A tile set, 48 chunks: A | H2 | H1 | S1 | P1 | As2 | dH | dO | dOs | dO2.  dS1 and dP1 are written in place over S1 and P1 (the
+// B1 epilogue reads each mask element and writes the gradient element of the same thread and offset), once the weight-gradient
+// GEMMs that read S1 and P1 are complete.  dH holds dH2, then dH1.  The wgrad GEMMs' 64-column MN-major reads of the narrower
+// tiles S1, P1 and As2 run on into the next tiles of the set; the rows they produce there are never used.
 constexpr uint32_t B_W = 0;
-constexpr uint32_t B_ACT = B_W + W_BYTES;            // activations, 34 chunks: A | H2 | H1 | S1 | P1 | As2
-constexpr uint32_t A_A = 0, A_H2 = 16384, A_H1 = 32768, A_S1 = 49152, A_P1 = 57344, A_AS2 = 65536, ACT_BYTES = 69632;
-constexpr uint32_t B_GRAD = B_ACT + ACT_BYTES;        // gradients: dH | dS1 | dP1 | dO | dOs | dO2
-constexpr uint32_t G_DH = 0, G_DS1 = 16384, G_DP1 = 24576, G_DO = 32768, G_DOS = 36864, G_DO2 = 40960, GRAD_BYTES = 45056;
-constexpr uint32_t B_BYTES = B_GRAD + GRAD_BYTES;    // 140288
+constexpr uint32_t T_A = 0, T_H2 = 16384, T_H1 = 32768, T_S1 = 49152, T_P1 = 57344, T_AS2 = 65536, T_DH = 69632, T_DO = 86016,
+                   T_DOS = 90112, T_DO2 = 94208, T_BYTES = 98304;
+constexpr uint32_t B_SET = B_W + W_BYTES;            // first tile set
 
-// constant-zero parts of the narrow backward tiles (their second K chunk, and unused columns of the first)
-__device__ __forceinline__ void zero_narrow_tiles(uint8_t* smem_base, uint32_t tid) {
-    uint8_t* act = smem_base + B_ACT; uint8_t* grd = smem_base + B_GRAD;
-    uint8_t* sP1 = act + A_P1; uint8_t* sAs2 = act + A_AS2;
-    uint8_t* sdP1 = grd + G_DP1; uint8_t* sdO = grd + G_DO; uint8_t* sdOs = grd + G_DOS; uint8_t* sdO2 = grd + G_DO2;
+// constant-zero parts of the narrow backward tiles (their second K chunk, and unused columns of the first), and the specular
+// tiles As2, P1 / dP1 and dO2, which only full shading writes
+__device__ __forceinline__ void zero_narrow_tiles(uint8_t* set, uint32_t tid) {
     const uint4 z = make_uint4(0, 0, 0, 0);
-    *reinterpret_cast<uint4*>(sAs2 + kChunk + tid * 16) = z;
-    *reinterpret_cast<uint4*>(sdO + kChunk + tid * 16) = z;
-    *reinterpret_cast<uint4*>(sdOs + kChunk + tid * 16) = z;
-    *reinterpret_cast<uint4*>(sdO2 + kChunk + tid * 16) = z;
-    *reinterpret_cast<uint4*>(sAs2 + tid * 16) = z;
+    *reinterpret_cast<uint4*>(set + T_AS2 + kChunk + tid * 16) = z;
+    *reinterpret_cast<uint4*>(set + T_DO + kChunk + tid * 16) = z;
+    *reinterpret_cast<uint4*>(set + T_DOS + kChunk + tid * 16) = z;
+    *reinterpret_cast<uint4*>(set + T_DO2 + kChunk + tid * 16) = z;
+    *reinterpret_cast<uint4*>(set + T_DO2 + tid * 16) = z;
+    *reinterpret_cast<uint4*>(set + T_AS2 + tid * 16) = z;
 #pragma unroll
-    for (int ch = 0; ch < 4; ++ch) {
-        *reinterpret_cast<uint4*>(sP1 + ch * kChunk + tid * 16) = z;
-        *reinterpret_cast<uint4*>(sdP1 + ch * kChunk + tid * 16) = z;
-    }
+    for (int ch = 0; ch < 4; ++ch) *reinterpret_cast<uint4*>(set + T_P1 + ch * kChunk + tid * 16) = z;
 }
 
 // ================================================================================================
-// one 128-sample tile of the MLPs on the warpgroup of threads 0..127 (wgmma, accumulators in registers)
+// one 128-sample tile of the MLPs on one warpgroup (wgmma, accumulators in registers)
 // ================================================================================================
 // The caller's `sync()` makes generic smem writes visible to the tensor core and meets all 128 threads at a barrier.
 // Every round waits for its MMAs; a barrier follows the wait where the epilogue overwrites a tile other warps' MMAs read.
@@ -221,19 +234,80 @@ struct WgradAcc {
     }
 };
 
-// backward of one tile (forward recompute, dgrad, wgrad).  dv: upstream gradient of this thread's sample (zero if not owned);
-// emit(d_enc) receives the 128 x 64 accumulator of the encoding gradient.
-template <class Sync, class Emit>
-__device__ __forceinline__ void mlp_bwd_tile(uint8_t* smem_base, float4 dv, bool own, bool full, float spec_reg, uint32_t tid,
-                                             WgradAcc& wa, Sync sync, Emit emit) {
-    uint8_t* sW = smem_base + B_W; uint8_t* act = smem_base + B_ACT; uint8_t* grd = smem_base + B_GRAD;
-    uint8_t* sA = act + A_A; uint8_t* sH2 = act + A_H2; uint8_t* sH1 = act + A_H1; uint8_t* sS1 = act + A_S1;
-    uint8_t* sP1 = act + A_P1; uint8_t* sAs2 = act + A_AS2;
-    uint8_t* sdH = grd + G_DH; uint8_t* sdS1 = grd + G_DS1; uint8_t* sdP1 = grd + G_DP1; uint8_t* sdO = grd + G_DO;
-    uint8_t* sdOs = grd + G_DOS; uint8_t* sdO2 = grd + G_DO2;
+// ---- the backward of one tile in two roles ---------------------------------------------------------------------------------
+// The chain (mlp_bwd_chain) runs the forward recompute, the per-sample chain rule and the dgrad GEMMs down to the encoding
+// gradient; it holds one round's accumulators at a time.  The weight gradients (mlp_wgrad_step) are GEMMs over the tile's
+// activation and gradient tiles, in five steps, each issued once the chain has written the tiles it reads:
+//     step 0 (after the chain rule): S1^T dOs, P1^T dO2                -> then S1 / P1 may be overwritten (dS1 / dP1 in place)
+//     step 1 (after B1): A^T dS1, As2^T dP1
+//     step 2 (after B2): H2^T dO
+//     step 3 (after B3): H1^T dH2                                       -> then dH may be overwritten (dH1)
+//     step 4 (after B4): A^T dH1                                        -> then the whole tile set is free
+// The chain calls hooks.ready(step) after the barrier that publishes a step's tiles, and hooks.released(what) before it overwrites
+// a tile that step 0 / step 3 read; released() returns once the weight-gradient MMAs of every warp that read the tile are
+// complete.  In the warp-specialised kernel ready() / released() are mbarrier arrivals / waits between the chain and a
+// weight-gradient warpgroup; a warpgroup that runs both roles issues the step from ready() and meets at its barrier in released().
+constexpr int kWgradSteps = 5;
+enum { REL_S1P1 = 0, REL_DH = 1, REL_SET = 2 };
+
+// weight-gradient step `step` of the tile in tile set `set`, issued and completed by the calling warpgroup
+// The specular GEMMs are issued in both shading modes (a wgmma under a branch makes ptxas fence the accumulator registers of the
+// whole group); without full shading their operand tiles stay zero, and nothing reads what they accumulate.
+__device__ __forceinline__ void mlp_wgrad_step(int step, const uint8_t* set, WgradAcc& wa) {
+    const uint8_t* sA = set + T_A; const uint8_t* sH2 = set + T_H2; const uint8_t* sH1 = set + T_H1;
+    const uint8_t* sS1 = set + T_S1; const uint8_t* sP1 = set + T_P1; const uint8_t* sAs2 = set + T_AS2;
+    const uint8_t* sdS1 = set + T_S1; const uint8_t* sdP1 = set + T_P1; const uint8_t* sdH = set + T_DH;
+    const uint8_t* sdO = set + T_DO; const uint8_t* sdOs = set + T_DOS; const uint8_t* sdO2 = set + T_DO2;
+    wg::wgmma_fence();
+    switch (step) {
+        case 0:
+            wg::gemm64<16, 8, true, true>(wa.s2, opMN(sS1, 128), opMN(sdOs, 128), true);             // rows 0..31: S1^T dOs
+            wg::gemm64<16, 8, true, true>(wa.p2, opMN(sP1, 128), opMN(sdO2, 128), true);             // rows 0..31: P1^T dO2
+            wg::commit(); wg::wait(wa.s2, wa.p2);
+            break;
+        case 1:
+            wg::gemm64<32, 8, true, true>(wa.s1, opMN(sA, 128), opMN(sdS1, 128), true);              // rows 0..63: A^T dS1
+            wg::gemm64<32, 8, true, true>(wa.p1, opMN(sAs2, 128), opMN(sdP1, 128), true);            // rows 0..5: As2^T dP1
+            wg::commit(); wg::wait(wa.s1, wa.p1);
+            break;
+        case 2:
+            wg::gemm64<16, 8, true, true>(wa.c3, opMN(sH2, 128), opMN(sdO, 128), true);              // rows 0..63: H2^T dO
+            wg::commit(); wg::wait(wa.c3);
+            break;
+        case 3:
+            wg::gemm64<64, 8, true, true>(wa.c2, opMN(sH1, 128), opMN(sdH, 128), true);              // rows 0..63: H1^T dH2
+            wg::commit(); wg::wait(wa.c2);
+            break;
+        default:
+            wg::gemm64<64, 8, true, true>(wa.c1, opMN(sA, 128), opMN(sdH, 128), true);               // rows 0..63: A^T dH1
+            wg::commit(); wg::wait(wa.c1);
+            break;
+    }
+}
+
+// both roles on one warpgroup: each weight-gradient step runs as soon as its tiles are published.  wgmma.wait_group waits for the
+// calling warp's share of the MMAs only, so before the chain overwrites a tile a step read (the B1 epilogue writes dS1 / dP1 over
+// S1 / P1 in every column of its warp's rows), the warpgroup meets at its barrier: every warp has then waited for its step MMAs.
+template <class Sync>
+struct InlineWgrad {
+    const uint8_t* set; WgradAcc& wa; Sync sync;
+    __device__ __forceinline__ void ready(int step) { mlp_wgrad_step(step, set, wa); }
+    __device__ __forceinline__ void released(int) { sync(); }
+};
+
+// chain role of the backward of one tile in tile set `set` (forward recompute, dgrad).  dv: upstream gradient of this thread's
+// sample (zero if not owned); emit(d_enc) receives the 128 x 64 accumulator of the encoding gradient.  `tid`: 0..127 in the
+// chain's warpgroup; `sync()` makes generic smem writes visible to the tensor core and meets the warpgroup's 128 threads.
+template <class Sync, class Hooks, class Emit>
+__device__ __forceinline__ void mlp_bwd_chain(const uint8_t* sW, uint8_t* set, float4 dv, bool own, bool full, float spec_reg,
+                                              uint32_t tid, Sync sync, Hooks& hooks, Emit emit) {
+    uint8_t* sA = set + T_A; uint8_t* sH2 = set + T_H2; uint8_t* sH1 = set + T_H1; uint8_t* sS1 = set + T_S1;
+    uint8_t* sP1 = set + T_P1; uint8_t* sAs2 = set + T_AS2;
+    uint8_t* sdH = set + T_DH; uint8_t* sdS1 = set + T_S1; uint8_t* sdP1 = set + T_P1; uint8_t* sdO = set + T_DO;
+    uint8_t* sdOs = set + T_DOS; uint8_t* sdO2 = set + T_DO2;
     const uint32_t r = sample_row(tid);
 
-    // ---------------- forward recompute (one layer per round: the wgrad accumulators hold 120 registers) ----------------
+    // ---------------- forward recompute (one layer per round, the rounds of the reference numerics) ----------------
     {
         float c[2][32];
         wg::wgmma_fence();
@@ -323,34 +397,29 @@ __device__ __forceinline__ void mlp_bwd_tile(uint8_t* smem_base, float4 dv, bool
         if (full) store_chunk(sdO2, 0, r, dO2);
     }
     sync();
+    hooks.ready(0);
 
-    // ---------------- B1: specular_net.1 / sigma_net.1 dgrad + their wgrads ----------------
+    // ---------------- B1: specular_net.1 / sigma_net.1 dgrad ----------------
     {
         float d[2][16], e[2][16];
         wg::wgmma_fence();
         wg::gemm128<32, 1, false, true>(d, opK(sdOs, 128), opMN(sW + W_S2, 16), false);           // dS1 (pre-mask)
-        wg::gemm64<16, 8, true, true>(wa.s2, opMN(sS1, 128), opMN(sdOs, 128), true);             // rows 0..31: S1^T dOs
-        if (full) {
-            wg::gemm128<32, 1, false, true>(e, opK(sdO2, 128), opMN(sW + W_P2, 16), false);       // dP1 (pre-mask)
-            wg::gemm64<16, 8, true, true>(wa.p2, opMN(sP1, 128), opMN(sdO2, 128), true);         // rows 0..31: P1^T dO2
-        }
-        wg::commit(); wg::wait(d, e, wa.s2, wa.p2);
+        wg::gemm128<32, 1, false, true>(e, opK(sdO2, 128), opMN(sW + W_P2, 16), false);           // dP1 (pre-mask)
+        wg::commit(); wg::wait(d, e);
+        hooks.released(REL_S1P1);                        // dS1 / dP1 overwrite S1 / P1
         epi_store<32, false>(d, sdS1, tid, sS1);
         if (full) epi_store<32, false>(e, sdP1, tid, sP1);
     }
     sync();
+    hooks.ready(1);
 
-    // ---------------- B2: sigma_net.0 wgrad, specular_net.0 dgrad + wgrad ----------------
+    // ---------------- B2: specular_net.0 dgrad ----------------
     {
         float e[2][8], v[8];
-        wg::wgmma_fence();
-        wg::gemm64<32, 8, true, true>(wa.s1, opMN(sA, 128), opMN(sdS1, 128), true);              // rows 0..63: A^T dS1
         if (full) {
+            wg::wgmma_fence();
             wg::gemm128<16, 2, false, true>(e, opK(sdP1, 128), opMN(sW + W_P1, 32), false);       // d As2
-            wg::gemm64<32, 8, true, true>(wa.p1, opMN(sAs2, 128), opMN(sdP1, 128), true);        // rows 0..5: As2^T dP1
-        }
-        wg::commit(); wg::wait(e, wa.s1, wa.p1);
-        if (full) {
+            wg::commit(); wg::wait(e);
             row_cols<16, 6>(e, v, tid);
             dfeat[3] = v[3]; dfeat[4] = v[4]; dfeat[5] = v[5];
         }
@@ -360,38 +429,39 @@ __device__ __forceinline__ void mlp_bwd_tile(uint8_t* smem_base, float4 dv, bool
         store_chunk(sdO, 0, r, dO);
     }
     sync();
+    hooks.ready(2);
 
-    // ---------------- B3: color_net.2 dgrad + wgrad ----------------
+    // ---------------- B3: color_net.2 dgrad ----------------
     {
         float d[2][32];
         wg::wgmma_fence();
         wg::gemm128<64, 1, false, true>(d, opK(sdO, 128), opMN(sW + W_C3, 16), false);            // dH2 (pre-mask)
-        wg::gemm64<16, 8, true, true>(wa.c3, opMN(sH2, 128), opMN(sdO, 128), true);              // rows 0..63: H2^T dO
-        wg::commit(); wg::wait(d, wa.c3);
+        wg::commit(); wg::wait(d);
         epi_store<64, false>(d, sdH, tid, sH2);
     }
     sync();
+    hooks.ready(3);
 
-    // ---------------- B4: color_net.1 dgrad + wgrad ----------------
+    // ---------------- B4: color_net.1 dgrad ----------------
     {
         float d[2][32];
         wg::wgmma_fence();
         wg::gemm128<64, 4, false, true>(d, opK(sdH, 128), opMN(sW + W_C2, 64), false);            // dH1 (pre-mask)
-        wg::gemm64<64, 8, true, true>(wa.c2, opMN(sH1, 128), opMN(sdH, 128), true);              // rows 0..63: H1^T dH2
-        wg::commit(); wg::wait(d, wa.c2);
+        wg::commit(); wg::wait(d);
         sync();                                          // dH1 overwrites dH2: every warp's MMAs have read it
+        hooks.released(REL_DH);
         epi_store<64, false>(d, sdH, tid, sH1);
     }
     sync();
+    hooks.ready(4);
 
-    // ---------------- B5: encoding dgrad (sigma_net.0 + color_net.0) + color_net.0 wgrad ----------------
+    // ---------------- B5: encoding dgrad (sigma_net.0 + color_net.0) ----------------
     {
         float d[2][32];
         wg::wgmma_fence();
         wg::gemm128<64, 2, false, true>(d, opK(sdS1, 128), opMN(sW + W_S1, 32), false);           // d enc  = dS1 W_s1
         wg::gemm128<64, 4, false, true>(d, opK(sdH, 128), opMN(sW + W_C1, 64), true);             // d enc += dH1 W_c1
-        wg::gemm64<64, 8, true, true>(wa.c1, opMN(sA, 128), opMN(sdH, 128), true);               // rows 0..63: A^T dH1
-        wg::commit(); wg::wait(d, wa.c1);
+        wg::commit(); wg::wait(d);
         emit(d);
     }
 }

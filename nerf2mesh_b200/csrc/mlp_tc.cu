@@ -3,14 +3,14 @@
 // in registers), operands staged in shared memory as core-matrix tiles, first-layer activations brought
 // in with one bulk async copy (TMA unit, cp.async.bulk) per 128-sample tile.
 //
-// Mapping: one CTA = one warpgroup of 128 threads = one 128-sample tile = the M dimension of every
+// Mapping: one warpgroup of 128 threads works on one 128-sample tile = the M dimension of every
 // forward / dgrad GEMM (two m64 halves).  Layer epilogues (ReLU, masks) work on the accumulator
 // fragments directly; the per-sample chain (sigmoid, exp, clamp, loss-side chain rule) runs one
 // sample per thread, its few columns gathered from the fragments by warp shuffles (mlp_common.cuh).
 // Weight gradients are GEMMs whose reduction dimension is the SAMPLE index; the same shared-memory
-// activation / gradient tiles are re-read MN-major for them (wg.cuh) and the accumulators stay
-// resident in registers across all tiles a persistent CTA processes, then are flushed once with
-// atomics.  Numerics follow torch.autocast(fp16): operands and layer outputs rounded to
+// activation / gradient tiles are re-read MN-major for them (wg.cuh).  In the backward kernel a
+// warpgroup of its own issues them, and its accumulators stay resident in registers across all
+// tiles a persistent CTA processes, then are flushed once with atomics.  Numerics follow torch.autocast(fp16): operands and layer outputs rounded to
 // fp16, fp32 accumulation; gradients are carried loss-scaled in fp16 like GradScaler does.
 #include "n2m_common.cuh"
 #include "mlp_common.cuh"
@@ -105,43 +105,73 @@ k_mlp_fwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const int32_t*
 // ================================================================================================
 // backward (forward recompute + dgrad + wgrad)
 // ================================================================================================
-// One CTA per SM: 255 registers per thread (-Xptxas -v, CUDA 12.9: 84 B of spills, and ptxas serialises some wgmma issues around
-// register use, C7519).  On an H100 SXM 80 GB at 700 W the kernel takes 0.19 ms of the 1.33 ms lego step (bench.py, stage times).
-__global__ void __launch_bounds__(128, 1)
-k_mlp_bwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const float4* __restrict__ dout,
-          const int32_t* __restrict__ counters, const uint8_t* __restrict__ wpack, uint8_t* __restrict__ denc_tiles,
-          float* __restrict__ g_mlp, const float* __restrict__ loss_scale, uint32_t part, uint32_t nparts) {
-    extern __shared__ __align__(128) uint8_t smem[];
-    __shared__ uint64_t bar_tma;
-    const uint32_t tid = threadIdx.x;
-    // rows outside [lo, hi) of a boundary tile belong to a neighbouring part: zero upstream gradient (so they add
-    // nothing to the weight gradients; their activations are whatever finite values the tile holds) and no store
-    const PartRange pr = part_range(counters, part, nparts);
-    const uint32_t M = pr.M;
-    const uint32_t t0 = pr.lo / kTile, t1 = (pr.hi + kTile - 1) / kTile;
-    if (pr.hi <= pr.lo || t0 + blockIdx.x >= t1) return;
+// One CTA per SM of three warpgroups: two chain warpgroups (mlp_bwd_chain) work on alternating tiles of the CTA, each in its own
+// tile set, and one weight-gradient warpgroup runs the wgrad steps (mlp_wgrad_step) of both, tile after tile in the CTA's order,
+// holding the weight-gradient accumulators (WgradAcc, 120 fp32 registers per thread) across all of them.  While one chain waits on
+// a round's MMAs, a TMA load or a barrier, the other chain and the wgrad GEMMs use the tensor core.
+// Shared memory: 25,600 B of weights + 2 x 98,304 B tile sets = 222,208 B (+ 144 B of mbarriers).  Registers: 384 threads at
+// __launch_bounds__(384, 1), at most 168 per thread.
+// Hand-over per tile set (mbarriers, one phase per tile of the set; mbar_wait traps instead of hanging):
+//   ready[s][k]  chain -> wgrad, 1 arrival (chain thread 0, after the barrier that publishes step k's tiles);
+//                the wgrad warpgroup waits for phase `it` of its it-th tile of the set
+//   rel[s][0]    wgrad -> chain, 128 arrivals, after step 0 (S1, P1 free): the chain waits for phase `it` of its own tile
+//   rel[s][1]    wgrad -> chain, 128 arrivals, after step 3 (dH2 free): as rel[s][0]
+//   rel[s][2]    wgrad -> chain, 128 arrivals, after step 4 (the tile set free): the chain waits for phase it - 1 before it
+//                loads its next tile (parity (it & 1) ^ 1, which a fresh barrier passes at it = 0)
+// A barrier never runs more than one phase ahead of its waiter: the chain's arrivals of tile it + 1 of a set follow its wait on
+// rel[s][2] of tile it, which follows the wgrad warpgroup's last wait on that set's ready barriers of tile it.
+// -Xptxas -v (CUDA 12.9, sm_90a): 159 registers, no stack frame, no spills, no wgmma serialisation advisories
+// (tests/test_mlp_bwd_compile.py keeps it so).  On an H100 80GB HBM3 at 700 W, on bench.py's lego batch (2.85e5 samples):
+// 80 us per launch against 180 us for the single-warpgroup kernel it replaces (profiles/mlp_bwd_time.py), 0.086 against
+// 0.193 ms as bench.py's cold-L2 stage time, and the lego step 1.272 against 1.334 ms.
+constexpr uint32_t kBwdChains = 2, kBwdThreads = 128 * (kBwdChains + 1);
+constexpr uint32_t B_BYTES = B_SET + kBwdChains * T_BYTES;            // 222,208
 
-    if (tid == 0) { wg::mbar_init(&bar_tma, 1); wg::mbar_init_fence(); }
-    for (uint32_t i = tid; i < W_BYTES / 16; i += 128)
-        reinterpret_cast<uint4*>(smem + B_W)[i] = __ldg(reinterpret_cast<const uint4*>(wpack) + i);
-    zero_narrow_tiles(smem, tid);
-    sync_before_mma();
-    uint32_t ph_tma = 0;
+// chain warpgroup c: make generic smem writes visible to the tensor core, meet the warpgroup's 128 threads at named barrier 1 + c.
+// One code path serves both chains (two inlined copies would let the compiler hoist their common descriptor arithmetic above the
+// role branch and hold it in registers through both); the register barrier id makes ptxas reserve all 16 named barriers.
+struct SyncChain {
+    uint32_t id;
+    __device__ __forceinline__ void operator()() const {
+        wg::fence_async_smem();
+        asm volatile("bar.sync %0, 128;" :: "r"(id) : "memory");
+    }
+};
+
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" :: "r"(wg::smem_u32(bar)) : "memory");
+}
+
+struct BwdBars {
+    uint64_t tma[kBwdChains], ready[kBwdChains][kWgradSteps], rel[kBwdChains][REL_SET + 1];
+};
+
+// chain side of the hand-over for the it-th tile of tile set s
+struct ChainHandover {
+    BwdBars* b; uint32_t s, it, tid;
+    __device__ __forceinline__ void ready(int step) { if (tid == 0) mbar_arrive(&b->ready[s][step]); }
+    __device__ __forceinline__ void released(int what) { wg::mbar_wait(&b->rel[s][what], it & 1); }
+};
+
+__device__ __forceinline__ void mlp_bwd_chain_role(uint32_t c, const n2m_s0_params& p, const uint8_t* __restrict__ enc_tiles,
+                                                   const float4* __restrict__ dout, uint8_t* __restrict__ denc_tiles, const PartRange& pr,
+                                                   uint32_t t0, uint32_t t1, uint32_t nparts, float spec_reg, uint8_t* smem, BwdBars* bars) {
+    const uint32_t tid = threadIdx.x & 127u;
     const bool full = p.shading_full != 0;
-    const float ls = loss_scale[0];
-    const float spec_reg = (M > 0) ? 2.0f * p.lambda_specular / (float)M * ls : 0.f;   // d/dspec of lambda * mean_j sum_c spec^2
     const uint32_t r = sample_row(tid);
-    WgradAcc wa;
-    wa.zero();
-
-    for (uint32_t tile = t0 + blockIdx.x; tile < t1; tile += gridDim.x) {
-        if (tid == 0) bulk_g2s(smem + B_ACT + A_A, enc_tiles + (size_t)tile * kTileBytes, kTileBytes, &bar_tma);
+    uint8_t* set = smem + B_SET + c * T_BYTES;
+    const SyncChain sync{1 + c};
+    uint32_t it = 0;
+    for (uint32_t tile = t0 + blockIdx.x + c * gridDim.x; tile < t1; tile += kBwdChains * gridDim.x, ++it) {
+        wg::mbar_wait(&bars->rel[c][REL_SET], (it & 1) ^ 1);        // the wgrad steps of this set's previous tile are complete
+        if (tid == 0) bulk_g2s(set + T_A, enc_tiles + (size_t)tile * kTileBytes, kTileBytes, &bars->tma[c]);
         const uint32_t j = tile * kTile + r;
         float4 dv = make_float4(0.f, 0.f, 0.f, 0.f);
         const bool own = j >= pr.lo && j < pr.hi;
         if (own) dv = dout[j];
-        wg::mbar_wait(&bar_tma, ph_tma); ph_tma ^= 1;
-        mlp_bwd_tile(smem, dv, own, full, spec_reg, tid, wa, sync_before_mma, [&](const float (&d)[2][32]) {
+        wg::mbar_wait(&bars->tma[c], it & 1);
+        ChainHandover h{bars, c, it, tid};
+        mlp_bwd_chain(smem + B_W, set, dv, own, full, spec_reg, tid, sync, h, [&](const float (&d)[2][32]) {
             // the feature gradients -> the tile's rows of the denc tile image (global)
             uint8_t* img = denc_tiles + (size_t)tile * kTileBytes;
 #pragma unroll
@@ -153,9 +183,63 @@ k_mlp_bwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const float4* 
                         *reinterpret_cast<uint32_t*>(img + wg::tile_off(row, frag_col(i, tid), kTile)) = pack2(d[hh][i], d[hh][i + 1]);
                 }
         });
-        sync_before_mma();
+        // every chain warp's B5 MMAs have read dS1 (in S1) and dH1 before the next tile's recompute writes S1 and H1 and its
+        // epilogues write dH
+        sync();
     }
-    flush_wgrad(wa, g_mlp, full, tid);
+}
+
+__global__ void __launch_bounds__(kBwdThreads, 1)
+k_mlp_bwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const float4* __restrict__ dout,
+          const int32_t* __restrict__ counters, const uint8_t* __restrict__ wpack, uint8_t* __restrict__ denc_tiles,
+          float* __restrict__ g_mlp, const float* __restrict__ loss_scale, uint32_t part, uint32_t nparts) {
+    extern __shared__ __align__(128) uint8_t smem[];
+    __shared__ BwdBars bars;
+    const uint32_t tid = threadIdx.x, wgi = tid >> 7;
+    // rows outside [lo, hi) of a boundary tile belong to a neighbouring part: zero upstream gradient (so they add
+    // nothing to the weight gradients; their activations are whatever finite values the tile holds) and no store
+    const PartRange pr = part_range(counters, part, nparts);
+    const uint32_t M = pr.M;
+    const uint32_t t0 = pr.lo / kTile, t1 = (pr.hi + kTile - 1) / kTile;
+    if (pr.hi <= pr.lo || t0 + blockIdx.x >= t1) return;
+
+    if (tid == 0) {
+        for (uint32_t c = 0; c < kBwdChains; ++c) {
+            wg::mbar_init(&bars.tma[c], 1);
+            for (int k = 0; k < kWgradSteps; ++k) wg::mbar_init(&bars.ready[c][k], 1);
+            for (int k = 0; k <= REL_SET; ++k) wg::mbar_init(&bars.rel[c][k], 128);
+        }
+        wg::mbar_init_fence();
+    }
+    for (uint32_t i = tid; i < W_BYTES / 16; i += kBwdThreads)
+        reinterpret_cast<uint4*>(smem + B_W)[i] = __ldg(reinterpret_cast<const uint4*>(wpack) + i);
+    if (wgi < kBwdChains) zero_narrow_tiles(smem + B_SET + wgi * T_BYTES, tid & 127u);
+    sync_before_mma();
+    const bool full = p.shading_full != 0;
+    const float ls = loss_scale[0];
+    const float spec_reg = (M > 0) ? 2.0f * p.lambda_specular / (float)M * ls : 0.f;   // d/dspec of lambda * mean_j sum_c spec^2
+
+    if (wgi < kBwdChains) {
+        mlp_bwd_chain_role(wgi, p, enc_tiles, dout, denc_tiles, pr, t0, t1, nparts, spec_reg, smem, &bars);
+    } else {
+        // weight-gradient warpgroup (the last one): the CTA's tiles in order, tile k in set k % kBwdChains
+        WgradAcc wa;
+        wa.zero();
+        uint32_t k = 0;
+        for (uint32_t tile = t0 + blockIdx.x; tile < t1; tile += gridDim.x, ++k) {
+            const uint32_t s = k % kBwdChains, par = (k / kBwdChains) & 1;
+            const uint8_t* set = smem + B_SET + s * T_BYTES;
+#pragma unroll
+            for (int step = 0; step < kWgradSteps; ++step) {
+                wg::mbar_wait(&bars.ready[s][step], par);
+                mlp_wgrad_step(step, set, wa);
+                if (step == 0) mbar_arrive(&bars.rel[s][REL_S1P1]);
+                if (step == 3) mbar_arrive(&bars.rel[s][REL_DH]);
+                if (step == 4) mbar_arrive(&bars.rel[s][REL_SET]);
+            }
+        }
+        flush_wgrad(wa, g_mlp, full, tid & 127u);
+    }
 }
 
 
@@ -215,7 +299,7 @@ int n2m_s0_mlp_bwd_part(const n2m_s0_params* p, const void* enc_tiles, const voi
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_mlp_bwd", "Mcap must be a positive multiple of 128");
     N2M_REQUIRE(valid_parts(part, nparts), "s0_mlp_bwd", "nparts must be 1, 2, 4 or 8 and part < nparts");
     const uint32_t grid = min(Mcap / kTile, (uint32_t)num_sms());
-    k_mlp_bwd<<<grid, 128, B_BYTES, as_stream(stream)>>>(*p, static_cast<const uint8_t*>(enc_tiles), static_cast<const float4*>(dout),
+    k_mlp_bwd<<<grid, kBwdThreads, B_BYTES, as_stream(stream)>>>(*p, static_cast<const uint8_t*>(enc_tiles), static_cast<const float4*>(dout),
                                                          counters, static_cast<const uint8_t*>(wpack), static_cast<uint8_t*>(denc_tiles),
                                                          g_mlp, loss_scale, part, nparts);
     return check_launch("s0_mlp_bwd");

@@ -198,8 +198,9 @@ class Stage0Trainer:
         self.params = S0Params()
         self._fill_params(shading_full=True, gt_has_alpha=True)
         # True: MLP backward + scatter as one warp-specialised launch (csrc/fused.cu); False: two launches.  The two launches are the
-        # faster choice on the H100 (H100 SXM 80 GB, 700 W: 1.33 against 1.41 ms per lego step in bench.py): the fused kernel's 640
-        # threads leave its MLP warps 96 registers at compile time, beside 120 registers of weight-gradient accumulators.
+        # faster choice on the H100 (H100 80GB HBM3, 700 W: 1.27 against 1.33 ms per lego step in bench.py): k_mlp_bwd keeps two
+        # tiles in flight per SM beside a weight-gradient warpgroup, while the fused kernel's 640 threads leave its one MLP warpgroup
+        # 96 registers at compile time, beside 120 registers of weight-gradient accumulators.
         self.fused_bwd = False
         self.fused_fwd = False              # True: gather + MLP forward as one warp-specialised launch (whole batch: needs nparts == 1)
         self.use_cam_near_far = False       # clamp (near, far) with the per-ray values in the slot's cam_nf (--enable_cam_near_far)

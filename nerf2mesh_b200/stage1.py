@@ -21,6 +21,7 @@ import torch
 from . import _lib
 from ._lib import F, I, P, U, call, ptr, stream
 from . import raster as dr
+from . import texture  # noqa: F401  (the stage-1 export, texture.export_stage1; binds include/n2m_b200_texture.h)
 from .stage0 import S0Params
 
 _lib.register({

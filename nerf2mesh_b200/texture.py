@@ -1,0 +1,237 @@
+"""Stage-1 export: the textured mesh of NeRFRenderer.export_stage1 (nerf/renderer.py:298-468) on the device.
+Host side of csrc/texture.cu (C ABI include/n2m_b200_texture.h).
+
+    vt, ft = <xatlas UV unwrap of (vertices, triangles)>                  # CPU, the caller's (see INTEGRATION.md 3d)
+    export_stage1(s1, save_path, vt, ft, resolution=4096)                 # -> mesh_0.obj, mesh_0.mtl, feat0_0.jpg, feat1_0.jpg, mlp.json
+
+The stages, each callable on its own:
+    uv_features(t0, vertices, triangles, vt, ft, h, w)  UV raster (n2m_rasterize of (vt * 2 - 1, 0, 1) / ft), positions interpolated with
+                                                        the position triangles, hash-grid gather, geo_feat on tensor cores, quantised:
+                                                        -> feats [h,w,6] uint8, mask [h,w] bool       (renderer.py:329-376)
+    inpaint(feats, mask)                                the 32-texel gutter from the nearest boundary texels, in place  (:378-394)
+    downscale(feats, ssaa)                              -> feat0, feat1 [h/ssaa, w/ssaa, 3] uint8 RGB                    (:396-402)
+    bake_features(...)                                  the three in a row
+    write_obj / write_mtl / write_mlp_json              the files (:409-439, :454-468)
+
+Everything up to the JPEG encode stays on the device; the only host copies are the two finished textures.  A mesh that covers no texel
+gives zero textures (the reference fails in its nearest-neighbour fit there).
+"""
+import json
+import os
+
+import numpy as np
+import torch
+
+from . import _lib
+from . import raster as dr
+from . import stage0  # noqa: F401  (binds the stage-0 gather n2m_s0_encode_points)
+from ._lib import P, U, call, ptr, stream
+
+_lib.register({
+    "n2m_s1_bake_points": [P, P, P, U, U, U, U, U, P, P, P, P],
+    "n2m_s1_geo_feat": [P, P, U, P, P, P, P, P],
+    "n2m_s1_inpaint": [P, P, U, U, P, P, P],
+    "n2m_s1_ssaa_down2": [P, U, U, U, P, P, P],
+})
+
+MAX_BAND_POINTS = 1 << 22          # points per band: 512 MiB of gather tiles (128 B per point) + 64 MiB of positions and texel indices
+
+
+def _as_tensor(x, dtype, device):
+    if not torch.is_tensor(x):
+        x = torch.from_numpy(np.ascontiguousarray(x))
+    return x.to(device=device, dtype=dtype).contiguous()
+
+
+def validate_mesh(vertices, triangles, vt, ft, h, w):
+    """ValueError unless ft matches triangles row for row, every index is in range, vt lies in [0, 1] and h * w fits the rasterizer."""
+    V, T = int(vertices.shape[0]), int(vt.shape[0])
+    if triangles.dim() != 2 or triangles.shape[1] != 3 or ft.dim() != 2 or ft.shape[1] != 3:
+        raise ValueError("triangles and ft must be [F,3]")
+    if ft.shape[0] != triangles.shape[0]:
+        raise ValueError(f"ft has {ft.shape[0]} rows, triangles {triangles.shape[0]}: one UV triangle per mesh triangle")
+    if vt.dim() != 2 or vt.shape[1] != 2:
+        raise ValueError("vt must be [Nt,2]")
+    if h <= 0 or w <= 0 or h * w >= 1 << 31:
+        raise ValueError(f"texture {h}x{w}: the UV raster holds fewer than 2^31 texels")
+    if ft.numel():
+        if int(ft.min()) < 0 or int(ft.max()) >= T:
+            raise ValueError(f"ft indexes outside vt (0..{T - 1})")
+        if int(triangles.min()) < 0 or int(triangles.max()) >= V:
+            raise ValueError(f"triangles index outside the vertices (0..{V - 1})")
+    if vt.numel() and not (bool(torch.isfinite(vt).all()) and float(vt.min()) >= 0.0 and float(vt.max()) <= 1.0):
+        raise ValueError("vt must lie in [0, 1]")
+
+
+class Baker:
+    """Band buffers of the feature bake: the points of `band_points` texels at a time (positions, texel indices, gather tiles)."""
+
+    def __init__(self, t0, band_points):
+        self.t0 = t0
+        dev = t0.device
+        self.cap = (int(band_points) + 127) // 128 * 128
+        self.pix = torch.zeros(self.cap, dtype=torch.int32, device=dev)
+        self.pts = torch.zeros(self.cap, 3, device=dev)
+        self.enc_tiles = torch.zeros(self.cap * 64, dtype=torch.float16, device=dev)
+        self.counters = torch.zeros(16, dtype=torch.int32, device=dev)
+
+    def band(self, rast, vertices, triangles, w, y0, y1, feats, feats_f32=None, contract=False):
+        """rows [y0, y1) of the UV raster: points -> gather -> geo_feat into feats [h*w*6] uint8 (feats_f32 [cap,6]: the float features of
+        the band's points, in the order of self.pix / self.pts)."""
+        self.points(rast, vertices, triangles, w, y0, y1, contract)
+        self.features(feats, feats_f32)
+
+    def points(self, rast, vertices, triangles, w, y0, y1, contract=False):
+        """the band's covered texels -> self.pix, self.pts, then the hash-grid gather of those points -> self.enc_tiles"""
+        t0 = self.t0
+        call("n2m_s1_bake_points", ptr(rast), ptr(vertices), ptr(triangles), w, y0, y1, self.cap, int(bool(contract)), ptr(self.counters),
+             ptr(self.pix), ptr(self.pts), stream())
+        call("n2m_s0_encode_points", t0._pp(), ptr(self.pts), None,
+             ptr(self.counters), self.cap, ptr(t0.table), ptr(t0.offsets), ptr(self.enc_tiles), stream())
+
+    def features(self, feats, feats_f32=None):
+        """geo_feat of the gathered points, quantised into their texels of feats"""
+        call("n2m_s1_geo_feat", ptr(self.enc_tiles), ptr(self.counters), self.cap, ptr(self.t0.wpack), ptr(self.pix), ptr(feats),
+             ptr(feats_f32), stream())
+
+
+def uv_raster(vertices_uv, ft, h, w, glctx=None):
+    """dr.rasterize of the atlas: clip positions (vt * 2 - 1, 0, 1), triangles ft, resolution (h, w) (renderer.py:329-338)"""
+    uv = vertices_uv * 2.0 - 1.0
+    clip = torch.cat((uv, torch.zeros_like(uv[:, :1]), torch.ones_like(uv[:, :1])), dim=-1).contiguous()
+    rast, _ = dr.rasterize(glctx or dr.RasterizeCudaContext(vertices_uv.device), clip, ft, (h, w))
+    return rast
+
+
+def uv_features(t0, vertices, triangles, vt, ft, h, w, band_rows=None, contract=None):
+    """-> feats [h,w,6] uint8 (geo_feat * 255 truncated at the covered texels, 0 elsewhere), mask [h,w] bool (covered texels).
+    `band_rows`: rows per bake band (default: as many as keep a band within MAX_BAND_POINTS texels)."""
+    dev = t0.device
+    vertices = _as_tensor(vertices, torch.float32, dev); triangles = _as_tensor(triangles, torch.int32, dev)
+    vt = _as_tensor(vt, torch.float32, dev); ft = _as_tensor(ft, torch.int32, dev)
+    h, w = int(h), int(w)
+    validate_mesh(vertices, triangles, vt, ft, h, w)
+    contract = t0.cfg.contract if contract is None else bool(contract)
+    rast = uv_raster(vt, ft, h, w)
+    mask = rast[0, ..., 3] > 0
+    feats = torch.zeros(h, w, 6, dtype=torch.uint8, device=dev)
+    rows = int(band_rows) if band_rows else max(1, MAX_BAND_POINTS // w)
+    rows = max(1, min(rows, h))
+    baker = Baker(t0, rows * w)
+    overflow = torch.zeros(1, dtype=torch.int32, device=dev)
+    for y0 in range(0, h, rows):
+        baker.band(rast, vertices, triangles, w, y0, min(h, y0 + rows), feats, contract=contract)
+        overflow += baker.counters[2:3]
+    if int(overflow.item()) != 0:         # a band holds at most cap texels: cannot happen unless the buffers were resized
+        raise RuntimeError("uv_features: point buffer overflow")
+    return feats, mask
+
+
+def inpaint(feats, mask, return_source=False):
+    """In place on feats [h,w,6] uint8: the gutter texels (within L1 distance 32 of the mask) copy their Euclidean-nearest boundary texel
+    (mask texels within L1 distance 3 of a non-mask texel or of the border); all other non-mask texels become 0.  Ties: smallest row, then
+    smallest column of the source.  return_source: also the source texel index per texel (int32 [h,w], -1 where nothing is copied)."""
+    h, w = int(feats.shape[0]), int(feats.shape[1])
+    if feats.dtype != torch.uint8 or tuple(feats.shape) != (h, w, 6) or not feats.is_contiguous() or not feats.is_cuda:
+        raise ValueError("inpaint: feats must be a contiguous CUDA uint8 tensor [h,w,6]")
+    m = mask.to(feats.device).reshape(h, w).to(torch.uint8).contiguous()
+    scratch = torch.empty(3 * h * w, dtype=torch.uint8, device=feats.device)
+    src = torch.empty(h, w, dtype=torch.int32, device=feats.device) if return_source else None
+    call("n2m_s1_inpaint", ptr(feats), ptr(m), h, w, ptr(scratch), ptr(src), stream())
+    return (feats, src) if return_source else feats
+
+
+def downscale(feats, ssaa):
+    """feats [h,w,6] uint8 -> (feat0, feat1) [h/ssaa, w/ssaa, 3] uint8 RGB: channels 0-2 and 3-5; ssaa 2 averages 2x2 blocks as
+    (a + b + c + d + 2) >> 2, which is cv2.resize(INTER_LINEAR) at exactly half size; ssaa 1 splits only."""
+    ssaa = int(ssaa)
+    if ssaa not in (1, 2):
+        raise ValueError("ssaa must be 1 or 2")
+    h, w = int(feats.shape[0]), int(feats.shape[1])
+    if h % ssaa or w % ssaa:
+        raise ValueError("the feature image is not a multiple of ssaa")
+    h0, w0 = h // ssaa, w // ssaa
+    feats = feats.contiguous()
+    feat0 = torch.empty(h0, w0, 3, dtype=torch.uint8, device=feats.device); feat1 = torch.empty_like(feat0)
+    call("n2m_s1_ssaa_down2", ptr(feats), h0, w0, ssaa, ptr(feat0), ptr(feat1), stream())
+    return feat0, feat1
+
+
+def bake_features(t0, vertices, triangles, vt, ft, h0, w0, ssaa=2, band_rows=None, contract=None):
+    """-> (feat0, feat1): the albedo and specular-feature textures, CUDA uint8 [h0,w0,3] RGB (renderer.py:329-402)."""
+    h, w = int(h0) * int(ssaa), int(w0) * int(ssaa)
+    feats, mask = uv_features(t0, vertices, triangles, vt, ft, h, w, band_rows=band_rows, contract=contract)
+    inpaint(feats, mask)
+    del mask
+    return downscale(feats, ssaa)
+
+
+# ---- files ----------------------------------------------------------------------------------------------------------------------
+def _np(x, dtype):
+    if torch.is_tensor(x):
+        x = x.detach().cpu().numpy()
+    return np.ascontiguousarray(x, dtype=dtype)
+
+
+def _rows(fmt, arr):
+    return "".join(fmt % tuple(r) for r in arr.tolist())
+
+
+def write_obj(path, v, f, vt, ft, mtl_name="mesh_0.mtl"):
+    """`v x y z`, `vt u (1 - v)`, `f a/at b/bt c/ct` (1-based), the layout of renderer.py:414-429.  Floats are float32 values written with
+    9 significant digits, which read back to the same float32."""
+    v = _np(v, np.float32); vt = _np(vt, np.float32); f = _np(f, np.int64); ft = _np(ft, np.int64)
+    vt_out = np.stack([vt[:, 0], np.float32(1) - vt[:, 1]], axis=1).astype(np.float32)       # float32 arithmetic, as the reference's
+    faces = np.stack([f[:, 0] + 1, ft[:, 0] + 1, f[:, 1] + 1, ft[:, 1] + 1, f[:, 2] + 1, ft[:, 2] + 1], axis=1)
+    with open(path, "w") as fp:
+        fp.write(f"mtllib {mtl_name} \n")
+        fp.write(_rows("v %.9g %.9g %.9g \n", v.astype(np.float64)))
+        fp.write(_rows("vt %.9g %.9g \n", vt_out.astype(np.float64)))
+        fp.write("usemtl defaultMat \n")
+        fp.write(_rows("f %d/%d %d/%d %d/%d \n", faces))
+
+
+def write_mtl(path, texture="feat0_0.jpg"):
+    """the material of renderer.py:431-439: map_Kd is the albedo texture"""
+    with open(path, "w") as fp:
+        fp.write("newmtl defaultMat \nKa 1 1 1 \nKd 1 1 1 \nKs 0 0 0 \nTr 1 \nillum 1 \nNs 0 \n")
+        fp.write(f"map_Kd {texture} \n")
+
+
+def specular_weights(t0):
+    """specular_net's weights {net.0.weight [32,6], net.1.weight [3,32]} (fp32) from the trainer's flat parameter vector"""
+    st = t0.export_reference_state()
+    return {k[len("specular_net."):]: st[k].detach().cpu().numpy() for k in ("specular_net.net.0.weight", "specular_net.net.1.weight")}
+
+
+def write_mlp_json(path, weights, bound, cascade=1):
+    """mlp.json of renderer.py:454-468: each specular_net weight transposed ([in, out]), `bound`, `cascade`"""
+    mlp = {k: np.asarray(p, dtype=np.float32).T.tolist() for k, p in weights.items()}
+    mlp["bound"] = float(bound)
+    mlp["cascade"] = int(cascade)
+    with open(path, "w") as fp:
+        json.dump(mlp, fp, indent=2)
+
+
+def write_textures(save_path, feat0, feat1, cas=0):
+    """feat0_<cas>.jpg / feat1_<cas>.jpg with cv2's default JPEG settings, BGR channel order (renderer.py:397-407)"""
+    import cv2
+    for name, img in ((f"feat0_{cas}.jpg", feat0), (f"feat1_{cas}.jpg", feat1)):
+        a = _np(img, np.uint8)
+        if not cv2.imwrite(os.path.join(save_path, name), np.ascontiguousarray(a[..., ::-1])):
+            raise RuntimeError(f"cv2.imwrite failed for {name}")
+
+
+def export_stage1(s1, save_path, vt, ft, resolution=4096, band_rows=None):
+    """NeRFRenderer.export_stage1 for one mesh (cascade 0) from a Stage1Trainer: vertices (base + offsets), triangles, the model of its
+    Stage0Trainer (call t0.ema_apply() first to export the EMA parameters), the trainer's ssaa; vt [Nt,2] / ft [F,3] from the caller's UV
+    unwrap.  Writes mesh_0.obj, mesh_0.mtl, feat0_0.jpg, feat1_0.jpg, mlp.json under save_path; returns (feat0, feat1) on the device."""
+    t0 = s1.t0
+    os.makedirs(save_path, exist_ok=True)
+    h0 = w0 = int(resolution)
+    feat0, feat1 = bake_features(t0, s1.vertices, s1.triangles, vt, ft, h0, w0, ssaa=s1.ssaa, band_rows=band_rows)
+    write_textures(save_path, feat0, feat1)
+    write_obj(os.path.join(save_path, "mesh_0.obj"), s1.vertices, s1.triangles, vt, ft)
+    write_mtl(os.path.join(save_path, "mesh_0.mtl"))
+    write_mlp_json(os.path.join(save_path, "mlp.json"), specular_weights(t0), bound=t0.cfg.bound, cascade=1)
+    return feat0, feat1

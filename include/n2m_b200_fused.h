@@ -200,18 +200,6 @@ int n2m_s0_encode_bwd_part(const n2m_s0_params* p, const void* recs, const int32
                            const int32_t* offsets, void* gtable, const float* loss_scale, uint32_t part, uint32_t nparts,
                            n2m_stream_t stream);
 
-/* Fused backward (csrc/fused.cu): MLP backward (wgmma) + hash-grid scatter of one part in ONE persistent, warp-specialised launch --
- * warps 0-3 run the MLP backward of a 128-sample tile, warps 4-19 scatter the previous tile's feature gradients, which are handed over
- * through a double-buffered shared-memory image instead of `denc_tiles` in HBM.  Same arithmetic as n2m_s0_mlp_bwd_part followed by
- * n2m_s0_encode_bwd_part (gradients equal up to fp32 atomic order); the TV gradient stays with n2m_s0_tv.  n2m_s0_fused_init sets the
- * kernel attributes once per process. */
-int n2m_s0_fused_init(void);
-/* profiling hook: bit 0 = scatter warps skip their REDs, bit 1 = MLP warps skip the tensor-core rounds (results meaningless) */
-int n2m_s0_set_fused_debug(int mode);
-int n2m_s0_bwd_fused_part(const n2m_s0_params* p, const void* enc_tiles, const void* dout, const void* recs, const int32_t* counters,
-                          uint32_t Mcap, const float* rays_o, const float* rays_d, const void* wpack, const int32_t* offsets,
-                          void* gtable, float* g_mlp, float* loss_scale, uint32_t part, uint32_t nparts, n2m_stream_t stream);
-
 /* optimizer state block (device, float[8]): [0] loss_scale, [1] growth_tracker, [2] adam step t,
  * [3] found_inf, [4] lr (host-written each step), [5] 1-beta1^t, [6] sqrt(1-beta2^t), [7] 1/loss_scale.
  * Every `loss_scale` pointer argument above is the base of this block: the kernels read [0] and set [3]
@@ -240,7 +228,8 @@ int n2m_s0_adam_post(float* opt_state, n2m_stream_t stream);
 /* Fused forward (csrc/fused.cu): hash-grid gather + MLP forward of the WHOLE batch (nparts == 1) in one persistent, warp-specialised
  * launch -- two gather groups of four warps fill double-buffered tile images in shared memory, warps 0-3 run the tensor-core MLP rounds on
  * them; a copy of every image is stored to enc_tiles by the TMA unit for the backward pass.  Same arithmetic as n2m_s0_encode_fwd followed
- * by n2m_s0_mlp_fwd (bit-identical enc_tiles / out). */
+ * by n2m_s0_mlp_fwd (bit-identical enc_tiles / out).  n2m_s0_fused_init sets the kernel attributes once per process. */
+int n2m_s0_fused_init(void);
 int n2m_s0_fwd_fused(const n2m_s0_params* p, const void* recs, const int32_t* counters, uint32_t Mcap, const float* rays_o,
                      const float* rays_d, const void* table, const int32_t* offsets, const void* wpack, void* enc_tiles, void* out,
                      float* spec_sq_sum, n2m_stream_t stream);

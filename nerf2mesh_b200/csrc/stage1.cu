@@ -9,7 +9,7 @@
 //   n2m_s0_encode_points, n2m_s0_mlp_fwd   self.rgb(x, d) (network.py:170-189) on tensor cores (sigma is computed and ignored)
 //   n2m_s1_loss                       alphas * rgbs, ssaa average (scale_img_hwc bilinear at factor 2 == 2x2 mean, :899-901), background
 //                                     mix (:907), MSE (+ mask) loss (utils.py:707-712) and its gradient w.r.t. every covered pixel's rgb
-//   n2m_s0_bwd_fused_part, n2m_s0_adam_*   backward of the colour MLPs + colour hash table, optimizer
+//   n2m_s0_mlp_bwd, n2m_s0_encode_bwd, n2m_s0_adam_*   backward of the colour MLPs + colour hash table, optimizer
 // With dr.antialias (renderer.py:886-887; csrc/antialias.cu) the middle of the step becomes
 //   n2m_s1_rgba                       scatter of the per-point colours into a full-resolution (r, g, b, mask) image (`rgbs[mask_flatten] =
 //                                     mask_rgbs`, `alphas = mask`, :881-884) -- ONE 4-channel image, so that one antialias launch serves both

@@ -66,8 +66,6 @@ _lib.register({
     "n2m_s0_adam_post": [P, P],
     "n2m_mark_untrained_grid": [P, U, P, U, P, F, P, F, U, U, P, P, P],
     "n2m_s0_fused_init": [],
-    "n2m_s0_set_fused_debug": [I],
-    "n2m_s0_bwd_fused_part": [PP, P, P, P, P, U, P, P, P, P, P, P, P, U, U, P],
     "n2m_s0_fwd_fused": [PP, P, P, U, P, P, P, P, P, P, P, P, P],
     "n2m_s0_render_begin": [PP, P, P, P, P, U, P, P, P, P, P, P, P, P],
     "n2m_s0_render_rounds": [PP, P, P, P, U, P, U, P, P, P, P, P, P, P, U, P, P, P, P, P, P, P],
@@ -197,11 +195,6 @@ class Stage0Trainer:
         self.loss_acc = torch.zeros(4, device=dev)          # [0] rgb(+mask) loss, [1] sum |spec|^2
         self.params = S0Params()
         self._fill_params(shading_full=True, gt_has_alpha=True)
-        # True: MLP backward + scatter as one warp-specialised launch (csrc/fused.cu); False: two launches.  The two launches are the
-        # faster choice on the H100 (H100 80GB HBM3, 700 W: 1.27 against 1.33 ms per lego step in bench.py): k_mlp_bwd keeps two
-        # tiles in flight per SM beside a weight-gradient warpgroup, while the fused kernel's 640 threads leave its one MLP warpgroup
-        # 96 registers at compile time, beside 120 registers of weight-gradient accumulators.
-        self.fused_bwd = False
         self.fused_fwd = False              # True: gather + MLP forward as one warp-specialised launch (whole batch: needs nparts == 1)
         self.use_cam_near_far = False       # clamp (near, far) with the per-ray values in the slot's cam_nf (--enable_cam_near_far)
         self._tv_overlap = True             # TV gradient as its own launch overlapped with the MLP kernels (tv mode 2)
@@ -245,6 +238,19 @@ class Stage0Trainer:
     @g_mlp.setter
     def g_mlp(self, t):
         self.g_mlps[min(self.parity, len(self.g_mlps) - 1)] = t
+
+    @property
+    def fused_bwd(self):
+        """Always False: the per-sample backward is two launches, k_mlp_bwd (two tiles in flight per SM beside a weight-gradient
+        warpgroup) and then the hash-grid scatter k_s0_encode_bwd.  The one-launch MLP-backward + scatter kernel was slower on every
+        workload on the H100 and has been removed; setting the flag to a true value raises ValueError, a false value is accepted."""
+        return False
+
+    @fused_bwd.setter
+    def fused_bwd(self, on):
+        if on:
+            raise ValueError("fused_bwd: the fused MLP-backward + scatter kernel was removed; the backward is k_mlp_bwd followed by "
+                             "k_s0_encode_bwd")
 
     @property
     def tv_overlap(self):
@@ -466,19 +472,6 @@ class Stage0Trainer:
         call("n2m_s0_fwd_fused", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
              ptr(self.table), ptr(self.offsets), ptr(self.wpack), ptr(self.enc_tiles), ptr(self.out), self.loss_acc.data_ptr() + 4, stream())
 
-    def bwd_fused(self, part=0, nparts=1):
-        call("n2m_s0_bwd_fused_part", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.recs), ptr(self.counters), self.Mcap,
-             ptr(self.rays_o), ptr(self.rays_d), ptr(self.wpack), ptr(self.offsets), ptr(self.gtables[self.parity]),
-             ptr(self.g_mlp), ptr(self.opt_state), part, nparts, stream())
-
-    def _backward(self, part=0, nparts=1):
-        """per-sample backward of one part on the current stream"""
-        if self.fused_bwd:
-            self.bwd_fused(part, nparts)
-        else:
-            self.mlp_bwd(part, nparts)
-            self.encode_bwd(part, nparts)
-
     def encode_bwd(self, part=0, nparts=1):
         call("n2m_s0_encode_bwd_part", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
              ptr(self.denc_tiles), ptr(self.table), ptr(self.offsets), ptr(self.gtables[self.parity]), ptr(self.opt_state),
@@ -538,8 +531,6 @@ class Stage0Trainer:
         P_ = int(self.nparts)
         has_tv = self.cfg.lambda_tv > 0
         fork_tv = self.tv_overlap and has_tv
-        if self.fused_bwd and has_tv and not fork_tv:
-            raise RuntimeError("fused_bwd evaluates no TV gradient: keep tv_overlap=True (TV as its own launch)")
 
         def launch_tv():
             if fork_tv:
@@ -560,7 +551,8 @@ class Stage0Trainer:
                 launch_tv()
                 self.mlp_fwd()
             self.composite_loss()
-            self._backward(0, 1)
+            self.mlp_bwd()
+            self.encode_bwd()
         else:
             # independent chains, one stream per part
             launch_tv()
@@ -574,7 +566,8 @@ class Stage0Trainer:
                     self.encode_fwd(k, P_)
                     self.mlp_fwd(k, P_)
                     self.composite_loss(k, P_)
-                    self._backward(k, P_)
+                    self.mlp_bwd(k, P_)
+                    self.encode_bwd(k, P_)
             for st in streams[1:]:
                 main.wait_stream(st)
         if fork_tv:
@@ -646,7 +639,7 @@ class Stage0Trainer:
             key = (name, self.parity)
         else:
             key = (name, self.cur, self.parity, int(self.params.shading_full), int(self.params.gt_has_alpha), int(self.nparts),
-                   bool(self.tv_overlap), bool(self.fused_bwd), bool(self.fused_fwd), int(self.tv_fallback_points), bool(self.defer_zero))
+                   bool(self.tv_overlap), bool(self.fused_fwd), int(self.tv_fallback_points), bool(self.defer_zero))
         g = self._graphs.get(key)
         if g is None:
             g = torch.cuda.CUDAGraph()

@@ -54,8 +54,8 @@ class Stage1Trainer:
         self.recs = torch.zeros(self.cap, 4, device=dev)
         self.counters = torch.zeros(16, dtype=torch.int32, device=dev)
         self.enc_tiles = torch.zeros(self.cap * 64, dtype=torch.float16, device=dev)
+        self.denc_tiles = torch.zeros(self.cap * 64, dtype=torch.float16, device=dev)
         self.out = torch.zeros(self.cap, 4, device=dev); self.dout = torch.zeros(self.cap, 4, device=dev)
-        self.denc_tiles = None               # only the two-kernel backward needs it (allocated on first use)
         Q = self.h0 * self.w0
         self.image = torch.zeros(Q, 3, device=dev); self.weights_sum = torch.zeros(Q, device=dev)
         self.loss_acc = torch.zeros(4, device=dev)
@@ -125,17 +125,10 @@ class Stage1Trainer:
         else:
             call("n2m_s1_loss", ptr(self.out), ptr(self.inv), ptr(gt), gt.shape[-1], ptr(bg), self.h0, self.w0, self.ssaa, self.lambda_mask,
                  ptr(t0.opt_state), ptr(self.dout), ptr(self.image), ptr(self.weights_sum), ptr(self.loss_acc), stream())
-        if t0.fused_bwd:
-            call("n2m_s0_bwd_fused_part", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.recs), ptr(self.counters), self.cap,
-                 ptr(self.pts), ptr(self.pdirs), ptr(t0.wpack), ptr(t0.offsets), ptr(t0.gtables[t0.parity]), ptr(t0.g_mlp),
-                 ptr(t0.opt_state), 0, 1, stream())
-        else:
-            if self.denc_tiles is None:
-                self.denc_tiles = torch.zeros(self.cap * 64, dtype=torch.float16, device=t0.device)
-            call("n2m_s0_mlp_bwd", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.cap, ptr(t0.wpack),
-                 ptr(self.denc_tiles), ptr(t0.g_mlp), ptr(t0.opt_state), stream())
-            call("n2m_s0_encode_bwd", self._pp(), ptr(self.recs), ptr(self.counters), self.cap, ptr(self.pts), ptr(self.pdirs),
-                 ptr(self.denc_tiles), ptr(t0.table), ptr(t0.offsets), ptr(t0.gtables[t0.parity]), ptr(t0.opt_state), stream())
+        call("n2m_s0_mlp_bwd", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.cap, ptr(t0.wpack),
+             ptr(self.denc_tiles), ptr(t0.g_mlp), ptr(t0.opt_state), stream())
+        call("n2m_s0_encode_bwd", self._pp(), ptr(self.recs), ptr(self.counters), self.cap, ptr(self.pts), ptr(self.pdirs),
+             ptr(self.denc_tiles), ptr(t0.table), ptr(t0.offsets), ptr(t0.gtables[t0.parity]), ptr(t0.opt_state), stream())
 
     def step(self, mvp, rays_d, gt, bg, shading="full", lr=None, use_graph=False):
         """One optimizer step on one view: mvp [4,4], rays_d [h0*w0,3] (unnormalised), gt [h0*w0, 3 or 4], bg [h0*w0,3].
@@ -154,7 +147,7 @@ class Stage1Trainer:
         else:
             if not (mvp.is_cuda and mvp.dtype == torch.float32 and mvp.is_contiguous()):
                 raise RuntimeError("use_graph: mvp must be a contiguous float32 CUDA tensor that stays in place (the graph is keyed by its address)")
-            key = (mvp.data_ptr(), rays_d.data_ptr(), gt.data_ptr(), bg.data_ptr(), int(gt.shape[-1]), shading, int(t0.parity), bool(t0.fused_bwd))
+            key = (mvp.data_ptr(), rays_d.data_ptr(), gt.data_ptr(), bg.data_ptr(), int(gt.shape[-1]), shading, int(t0.parity))
             g = self._graphs.get(key)
             if g is None:
                 g = torch.cuda.CUDAGraph()

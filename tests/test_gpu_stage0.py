@@ -215,37 +215,6 @@ def test_warp_marcher_equals_serial_marcher(name):
     assert torch.equal(s0[:M], s1[:M])
 
 
-@pytest.mark.parametrize("shading,n_rays,nparts", [("full", 192, 1), ("diffuse", 192, 1), ("full", 3072, 1), ("full", 3072, 2)])
-def test_fused_backward_equals_two_kernel_backward(shading, n_rays, nparts):
-    """k_s0_bwd_fused (MLP backward + scatter in one warp-specialised persistent launch, feature gradients handed over in shared
-    memory) vs k_mlp_bwd followed by k_s0_encode_bwd: same table / weight gradients up to the order of the fp32 atomics; 3072 rays give
-    every CTA several tiles (both buffers and both barrier phases are exercised), two parts exercise the boundary-tile row masks."""
-    tr, b = make(shading, N=n_rays)
-    tr.nparts = nparts
-    stage(tr, b)
-    tr._fill_params(shading == "full", True)
-    res = []
-    for fused in (False, True):
-        tr.fused_bwd = fused
-        tr.gtable.zero_(); tr.g_mlp.zero_(); tr.opt_state[3] = 0
-        tr.forward_backward()
-        torch.cuda.synchronize()
-        res.append({k: v.clone() for k, v in tr.export_reference_grads().items()})
-        assert tr.opt_state[3].item() == 0
-    M = int(tr.counters[1].item())
-    assert M > 128 * (torch.cuda.get_device_properties(0).multi_processor_count if n_rays > 1000 else 1)
-    for name in res[0]:
-        a, r = res[1][name].double(), res[0][name].double()
-        assert r.abs().max().item() > 0 or (shading == "diffuse" and name.startswith("specular")), name
-        assert (a - r).abs().max().item() <= 1e-4 * r.abs().max().item() + 1e-12, name
-    # the inf flag is raised by the fused kernel too
-    tr.gtable.zero_(); tr.g_mlp.zero_()
-    tr.opt_state[0] = 1e30
-    tr.forward_backward()
-    torch.cuda.synchronize()
-    assert tr.opt_state[3].item() == 1
-
-
 def test_update_density_grid_matches_reference_composition():
     """Stage0Trainer.update_density_grid vs the reference's update_extra_state arithmetic (renderer.py:1074-1149)
     composed from torch + the (bit-exact) operator-level encoder, same random jitter (one [H^3, 3] draw per cascade in the
@@ -334,7 +303,6 @@ def test_ray_range_parts_equal_whole_batch(nparts):
     both neighbours with row masks) give the same forward values exactly and the same loss / gradients up to fp32
     atomic summation order."""
     tr, b = make()
-    tr.fused_bwd = False          # the two-kernel backward leaves the feature gradients in denc_tiles, compared below
     stage(tr, b)
     tr.forward_backward()
     torch.cuda.synchronize()
@@ -552,7 +520,7 @@ def test_tv_random_point_fallback(ref_gridencoder):
 
 
 @pytest.mark.parametrize("shading,n_rays", [("full", 96), ("diffuse", 96), ("full", 4096)])
-def test_fused_forward_equals_two_kernel_forward(shading, n_rays):
+def test_fused_forward_equals_two_kernel_forward_and_trains_alike(shading, n_rays):
     """k_s0_fwd_fused (gather groups -> shared-memory tile image -> wgmma MLP rounds, TMA store of the image for the backward) vs
     k_s0_encode_fwd followed by k_mlp_fwd: bit-identical tile images and outputs (same per-sample arithmetic); 4096 rays give every CTA
     several tiles per gather group (buffer reuse, both barrier phases, the bulk-store read fence)."""
@@ -575,12 +543,12 @@ def test_fused_forward_equals_two_kernel_forward(shading, n_rays):
     assert torch.equal(res[0][0][: nt * 128 * 64], res[1][0][: nt * 128 * 64])
     assert torch.equal(res[0][1][:M], res[1][1][:M])
     assert abs(res[0][2] - res[1][2]) <= 1e-5 * max(abs(res[0][2]), 1e-12)
-    # and a whole step through the fused forward (+ fused backward) trains like the default path
+    # and a whole step through the fused forward trains like the default path
     losses = []
     for ff in (False, True):
         t2, b2 = make(seed=1, N=n_rays if n_rays < 1000 else 512)
         t2.nparts = 1
-        t2.fused_fwd = ff; t2.fused_bwd = ff
+        t2.fused_fwd = ff
         ls = []
         for it in range(3):
             t2.step(b2["ro"], b2["rd"], b2["gt"], b2["bg"], b2["noises"], use_graph=True)

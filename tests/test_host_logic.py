@@ -145,8 +145,8 @@ def test_peer_adam_slices_cover_rows_and_stay_aligned():
             assert lo[0] == 0 and hi[-1] == R and all(hi[r] == lo[r + 1] for r in range(W - 1))
 
 
-def test_step_orchestration_call_sequence(monkeypatch):
-    """Stage0Trainer's per-step orchestration (ray-range parts, TV fork, split optimizer, fused backward) with the CUDA layer mocked
+def test_step_orchestration_call_sequence_two_launch_backward(monkeypatch):
+    """Stage0Trainer's per-step orchestration (ray-range parts, TV fork, split optimizer, fused forward) with the CUDA layer mocked
     out: the sequence of C-ABI calls on every path, no GPU needed.  Guards the host logic that the GPU tests only exercise on a GPU."""
     import types
     import nerf2mesh_b200.stage0 as S0
@@ -190,11 +190,10 @@ def test_step_orchestration_call_sequence(monkeypatch):
     tr.params = S0.S0Params(); tr.Mcap, tr.N, tr.rows, tr.parity, tr.device = 128, 4, 160, 0, "cpu"
     tr._tv_overlap, tr._tv_stream, tr._part_streams = True, None, []
     tr._adam_stream = None
-    tr.fused_bwd, tr.fused_fwd, tr.tv_fallback_points, tr._graphs = False, False, 1000, {}
+    tr.fused_fwd, tr.tv_fallback_points, tr._graphs = False, 1000, {}
 
     tv = ["n2m_s0_tv", "n2m_s0_tv_random"]
     chain = ["n2m_s0_encode_fwd_part", "n2m_s0_mlp_fwd_part", "n2m_s0_composite_loss_part", "n2m_s0_mlp_bwd_part", "n2m_s0_encode_bwd_part"]
-    fchain = chain[:3] + ["n2m_s0_bwd_fused_part"]
     adam = ["n2m_s0_adam_head", "n2m_s0_adam_mlp", "n2m_s0_adam_tables", "n2m_s0_adam_post"]
 
     def names():
@@ -209,40 +208,34 @@ def test_step_orchestration_call_sequence(monkeypatch):
         assert names() == tv + chain * P_ + adam
         parts = [a[-3:-1] for n, a in calls if n == "n2m_s0_mlp_bwd_part"]
         assert parts == [(k, P_) for k in range(P_)]
-    # MLP backward + scatter as ONE launch (csrc/fused.cu)
-    calls.clear(); tr.fused_bwd, tr.nparts = True, 1
-    tr._compute_then_adam()
-    assert names() == [chain[0]] + tv + fchain[1:] + adam
-    calls.clear(); tr.nparts = 2
-    tr._compute_then_adam()
-    assert names() == tv + fchain * 2 + adam
+    # the backward is always MLP backward, then scatter: the fused backward is gone, and asking for it fails
+    import pytest
+    with pytest.raises(ValueError):
+        tr.fused_bwd = True
+    tr.fused_bwd = False
+    assert tr.fused_bwd is False
     # gather + MLP forward as one launch (whole batch only)
     calls.clear(); tr.fused_fwd, tr.nparts = True, 1
     tr._compute_then_adam()
-    assert names() == tv + ["n2m_s0_fwd_fused", chain[2], "n2m_s0_bwd_fused_part"] + adam
+    assert names() == tv + ["n2m_s0_fwd_fused"] + chain[2:] + adam
     tr.nparts = 2
-    import pytest
     with pytest.raises(RuntimeError):
         tr._compute()
     tr.fused_fwd = False
-    # TV inside the scatter kernel (tv mode 0): no TV launch, the fallback probe follows the scatter; not available with the fused backward
-    calls.clear(); tr.fused_bwd, tr.nparts = False, 1
+    # TV inside the scatter kernel (tv mode 0): no TV launch, the fallback probe follows the scatter
+    calls.clear(); tr.nparts = 1
     tr.tv_overlap = False
     assert names() == ["n2m_s0_set_tv_mode"]
     calls.clear()
     tr._compute_then_adam()
     assert names() == chain + ["n2m_s0_tv_random"] + adam
-    tr.fused_bwd = True
-    import pytest
-    with pytest.raises(RuntimeError):
-        tr._compute()
     # deferred zeroing of the gradient table: same launches, the optimizer variant that leaves the rows alone
-    calls.clear(); tr.defer_zero, tr.fused_bwd = True, False
+    calls.clear(); tr.defer_zero = True
     tr._compute_then_adam()
     assert names() == chain + ["n2m_s0_tv_random"] + adam[:2] + ["n2m_s0_adam_tables_keep", adam[3]]
     tr.defer_zero = False
     # lambda_tv == 0: no TV work at all
-    calls.clear(); tr.fused_bwd = False; tr.cfg.lambda_tv = 0.0
+    calls.clear(); tr.cfg.lambda_tv = 0.0
     tr._compute_then_adam()
     assert names() == chain + adam
 
@@ -329,7 +322,7 @@ def test_step_prefetch_ordering(monkeypatch):
     assert [(s, n) for s, k, n in log if k == "run"] == [("main", "march"), ("main", "compute+adam")]
 
 
-def test_stage1_step_call_sequences(monkeypatch):
+def test_stage1_step_call_sequences_two_launch_backward(monkeypatch):
     """Stage1Trainer._step_body with the CUDA layer mocked: plain, antialiased, and antialiased with the vertex-offset group (the check
     before the optimizer head, the group's update between the table sweep and the GradScaler update)"""
     import types
@@ -364,7 +357,7 @@ def test_stage1_step_call_sequences(monkeypatch):
     t0.cfg = types.SimpleNamespace(eps=1e-15)
     for k in ("table", "offsets", "opt_state", "wpack", "color_master", "m_table", "v_table", "mlp", "m_mlp", "v_mlp"):
         setattr(t0, k, torch.zeros(8))
-    t0.gtables, t0.g_mlps, t0.parity, t0.rows, t0._adam_stream, t0.fused_bwd, t0.global_step = [torch.zeros(8)] * 2, [torch.zeros(8)], 0, 8, None, True, 0
+    t0.gtables, t0.g_mlps, t0.parity, t0.rows, t0._adam_stream, t0.global_step = [torch.zeros(8)] * 2, [torch.zeros(8)], 0, 8, None, 0
     t0.params = S0.S0Params()
 
     def make(**kw):
@@ -373,19 +366,20 @@ def test_stage1_step_call_sequences(monkeypatch):
 
     mvp, rd, gt, bg = torch.eye(4), torch.rand(16, 3), torch.rand(16, 4), torch.rand(16, 3)
     fwd = ["n2m_rasterize", "n2m_s1_points", "n2m_s0_encode_points", "n2m_s0_mlp_fwd"]
+    bwd = ["n2m_s0_mlp_bwd", "n2m_s0_encode_bwd"]
     adam = ["n2m_s0_adam_head", "n2m_s0_adam_mlp", "n2m_s0_adam_tables", "n2m_s0_adam_post"]
     s1 = make()
     s1.step(mvp, rd, gt, bg)
-    assert calls == fwd + ["n2m_s1_loss", "n2m_s0_bwd_fused_part"] + adam and t0.global_step == 1
+    assert calls == fwd + ["n2m_s1_loss"] + bwd + adam and t0.global_step == 1
     calls.clear()
     s1 = make(antialias=True)
     s1.step(mvp, rd, gt, bg)
     aa_f, aa_b = ["n2m_s1_rgba", "n2m_antialias_forward"], ["n2m_s1_loss_aa", "n2m_antialias_backward", "n2m_s1_dout"]
-    assert calls == fwd + aa_f + aa_b + ["n2m_s0_bwd_fused_part"] + adam
+    assert calls == fwd + aa_f + aa_b + bwd + adam
     calls.clear()
     s1 = make(antialias=True, lr_vert=1e-4)
     s1.step(mvp, rd, gt, bg)
-    assert calls == fwd + aa_f + aa_b + ["n2m_s0_bwd_fused_part", "n2m_s1_vert_check"] + adam[:3] + ["n2m_s1_vert_step", adam[3]]
+    assert calls == fwd + aa_f + aa_b + bwd + ["n2m_s1_vert_check"] + adam[:3] + ["n2m_s1_vert_step", adam[3]]
     assert s1.vert_state[1].item() == pytest_approx(1e-4)
     # the image loss reaches the vertices through antialias only
     try:

@@ -113,24 +113,15 @@ k_s0_fwd_fused(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* 
 }
 
 }  // namespace
+
+cudaError_t fwd_fused_set_attributes() {
+    return cudaFuncSetAttribute(k_s0_fwd_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_BYTES);
+}
 }  // namespace n2m
 
 using namespace n2m;
 
-static int fused_num_sms() {
-    static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
-    return n;
-}
-
 extern "C" {
-
-int n2m_s0_fused_init(void) {
-    const cudaError_t e = cudaFuncSetAttribute(k_s0_fwd_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_BYTES);
-    if (e != cudaSuccess) return fail("s0_fused_init", cudaGetErrorString(e));
-    fused_num_sms();
-    return 0;
-}
 
 /* hash-grid gather + MLP forward of the WHOLE batch in one persistent launch (replaces n2m_s0_encode_fwd followed by n2m_s0_mlp_fwd):
  * the tile images go from the gather warps to the tensor core through shared memory; a copy is stored to enc_tiles (TMA bulk store) for
@@ -141,7 +132,7 @@ int n2m_s0_fwd_fused(const n2m_s0_params* p, const void* recs, const int32_t* co
     N2M_REQUIRE(p && recs && counters && rays_o && rays_d && table && offsets && wpack && enc_tiles && out, "s0_fwd_fused", "null pointer");
     N2M_REQUIRE(p->num_levels == kLevels, "s0_fwd_fused", "fused path supports num_levels == 16");
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_fwd_fused", "Mcap must be a positive multiple of 128");
-    const uint32_t grid = min(Mcap / kTile, (uint32_t)(2 * fused_num_sms()));
+    const uint32_t grid = min(Mcap / kTile, (uint32_t)(2 * num_sms()));
     k_s0_fwd_fused<<<grid, kFwdThreads, FF_BYTES, as_stream(stream)>>>(
         *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, static_cast<const TableEntry*>(table), offsets,
         static_cast<const uint8_t*>(wpack), static_cast<uint8_t*>(enc_tiles), static_cast<float4*>(out), spec_sq_sum);

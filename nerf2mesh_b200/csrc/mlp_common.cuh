@@ -199,4 +199,7 @@ __device__ __forceinline__ float4 mlp_fwd_tile(const uint8_t* sA, const uint8_t*
 }
 
 }  // namespace
+
+// dynamic shared memory opt-in of k_s0_fwd_fused (fused.cu); n2m_s0_init calls it with the attributes of the MLP kernels
+cudaError_t fwd_fused_set_attributes();
 }  // namespace n2m

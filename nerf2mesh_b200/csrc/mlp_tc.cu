@@ -537,24 +537,18 @@ int n2m_s0_pack_weights(const float* mlp_params, void* wpack, n2m_stream_t strea
     return check_launch("s0_pack_weights");
 }
 
-static int num_sms() {
-    static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
-    return n;
-}
-
-
-/* one-time function attributes (dynamic shared memory opt-in); safe to call repeatedly */
+/* one-time function attributes (dynamic shared memory opt-in) of every stage-0 kernel; safe to call repeatedly */
 int n2m_s0_init(void) {
     cudaError_t e = cudaFuncSetAttribute(k_mlp_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)F_BYTES);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(k_mlp_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)B_BYTES);
+    if (e == cudaSuccess) e = fwd_fused_set_attributes();
     if (e != cudaSuccess) return fail("s0_init", cudaGetErrorString(e));
     num_sms();
     return 0;
 }
 
-int n2m_s0_mlp_fwd_part(const n2m_s0_params* p, const void* enc_tiles, const int32_t* counters, uint32_t Mcap, const void* wpack,
-                        void* out, float* spec_sq_sum, uint32_t part, uint32_t nparts, n2m_stream_t stream) {
+int n2m_s0_mlp_fwd(const n2m_s0_params* p, const void* enc_tiles, const int32_t* counters, uint32_t Mcap, const void* wpack,
+                   void* out, float* spec_sq_sum, uint32_t part, uint32_t nparts, n2m_stream_t stream) {
     N2M_REQUIRE(p && enc_tiles && counters && wpack && out, "s0_mlp_fwd", "null pointer");
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_mlp_fwd", "Mcap must be a positive multiple of 128");
     N2M_REQUIRE(valid_parts(part, nparts), "s0_mlp_fwd", "nparts must be 1, 2, 4 or 8 and part < nparts");
@@ -565,14 +559,9 @@ int n2m_s0_mlp_fwd_part(const n2m_s0_params* p, const void* enc_tiles, const int
     return check_launch("s0_mlp_fwd");
 }
 
-int n2m_s0_mlp_fwd(const n2m_s0_params* p, const void* enc_tiles, const int32_t* counters, uint32_t Mcap, const void* wpack,
-                   void* out, float* spec_sq_sum, n2m_stream_t stream) {
-    return n2m_s0_mlp_fwd_part(p, enc_tiles, counters, Mcap, wpack, out, spec_sq_sum, 0, 1, stream);
-}
-
-int n2m_s0_mlp_bwd_part(const n2m_s0_params* p, const void* enc_tiles, const void* dout, const int32_t* counters, uint32_t Mcap,
-                        const void* wpack, void* denc_tiles, float* g_mlp, const float* loss_scale, uint32_t part, uint32_t nparts,
-                        n2m_stream_t stream) {
+int n2m_s0_mlp_bwd(const n2m_s0_params* p, const void* enc_tiles, const void* dout, const int32_t* counters, uint32_t Mcap,
+                   const void* wpack, void* denc_tiles, float* g_mlp, const float* loss_scale, uint32_t part, uint32_t nparts,
+                   n2m_stream_t stream) {
     N2M_REQUIRE(p && enc_tiles && dout && counters && wpack && denc_tiles && g_mlp && loss_scale, "s0_mlp_bwd", "null pointer");
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_mlp_bwd", "Mcap must be a positive multiple of 128");
     N2M_REQUIRE(valid_parts(part, nparts), "s0_mlp_bwd", "nparts must be 1, 2, 4 or 8 and part < nparts");
@@ -581,11 +570,6 @@ int n2m_s0_mlp_bwd_part(const n2m_s0_params* p, const void* enc_tiles, const voi
                                                          counters, static_cast<const uint8_t*>(wpack), static_cast<uint8_t*>(denc_tiles),
                                                          g_mlp, loss_scale, part, nparts);
     return check_launch("s0_mlp_bwd");
-}
-
-int n2m_s0_mlp_bwd(const n2m_s0_params* p, const void* enc_tiles, const void* dout, const int32_t* counters, uint32_t Mcap,
-                   const void* wpack, void* denc_tiles, float* g_mlp, const float* loss_scale, n2m_stream_t stream) {
-    return n2m_s0_mlp_bwd_part(p, enc_tiles, dout, counters, Mcap, wpack, denc_tiles, g_mlp, loss_scale, 0, 1, stream);
 }
 
 }  // extern "C"

@@ -36,6 +36,13 @@ inline cudaStream_t as_stream(n2m_stream_t s) { return reinterpret_cast<cudaStre
 template <typename T>
 __host__ __device__ inline T div_up(T a, T b) { return (a + b - 1) / b; }
 
+// SM count of the current device, read once per process (grid sizes of the persistent kernels)
+inline int num_sms() {
+    static int n = 0;
+    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
+    return n;
+}
+
 // ---- small device helpers ---------------------------------------------------------------------
 __device__ __forceinline__ float clampf(float x, float lo, float hi) { return fminf(hi, fmaxf(lo, x)); }
 

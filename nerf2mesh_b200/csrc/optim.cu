@@ -166,7 +166,7 @@ extern "C" int n2m_s0_pack_weights(const float* mlp_params, void* wpack, n2m_str
 extern "C" uint32_t n2m_s0_mlp_param_count(void);
 
 /* The optimizer stage in four launches.  adam_mlp (+ weight repack) and adam_tables are independent of each other (both only
- * READ opt_state), so a host may run them on two streams between head and post; n2m_s0_adam is the serial composition. */
+ * READ opt_state), so a host may run them on two streams between head and post. */
 extern "C" int n2m_s0_adam_head(const float* g_mlp, float* opt_state, n2m_stream_t stream) {
     N2M_REQUIRE(g_mlp && opt_state, "s0_adam_head", "null pointer");
     k_adam_head<<<1, 1024, 0, as_stream(stream)>>>(g_mlp, n2m_s0_mlp_param_count(), opt_state);
@@ -207,17 +207,6 @@ extern "C" int n2m_s0_adam_post(float* opt_state, n2m_stream_t stream) {
     N2M_REQUIRE(opt_state, "s0_adam_post", "null pointer");
     k_adam_post<<<1, 32, 0, as_stream(stream)>>>(opt_state);
     return check_launch("s0_adam(post)");
-}
-
-extern "C" int n2m_s0_adam(void* table, void* color_master, void* gtable, float* m_table, float* v_table, uint32_t rows,
-                           float* mlp_params, float* g_mlp, float* m_mlp, float* v_mlp, void* wpack, float* opt_state,
-                           float eps, n2m_stream_t stream) {
-    N2M_REQUIRE(table && color_master && gtable && m_table && v_table && mlp_params && g_mlp && m_mlp && v_mlp && wpack && opt_state,
-                "s0_adam", "null pointer");
-    if (int e = n2m_s0_adam_head(g_mlp, opt_state, stream)) return e;
-    if (int e = n2m_s0_adam_tables(table, color_master, gtable, m_table, v_table, rows, opt_state, eps, stream)) return e;
-    if (int e = n2m_s0_adam_mlp(mlp_params, g_mlp, m_mlp, v_mlp, wpack, opt_state, eps, stream)) return e;
-    return n2m_s0_adam_post(opt_state, stream);
 }
 
 

@@ -266,12 +266,6 @@ k_compact_covered(const float4* __restrict__ rast, const float* __restrict__ xyz
 
 using namespace n2m;
 
-static int raster_sms() {
-    static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
-    return n;
-}
-
 extern "C" {
 
 int n2m_rasterize(const float* pos, uint32_t V, const int32_t* tri, uint32_t F, uint32_t H, uint32_t W, void* vis, uint32_t* queue,
@@ -286,7 +280,7 @@ int n2m_rasterize(const float* pos, uint32_t V, const int32_t* tri, uint32_t F, 
     if (F > 0) {
         k_rast_small<<<div_up(F, 256u), 256, 0, st>>>(reinterpret_cast<const float4*>(pos), tri, F, H, W, static_cast<unsigned long long*>(vis), queue);
         if (int e = check_launch("rasterize(small)")) return e;
-        k_rast_large<<<raster_sms() * 8, 256, 0, st>>>(reinterpret_cast<const float4*>(pos), tri, H, W, static_cast<unsigned long long*>(vis), queue);
+        k_rast_large<<<num_sms() * 8, 256, 0, st>>>(reinterpret_cast<const float4*>(pos), tri, H, W, static_cast<unsigned long long*>(vis), queue);
         if (int e = check_launch("rasterize(large)")) return e;
     }
     k_rast_resolve<<<div_up(n, 256u), 256, 0, st>>>(reinterpret_cast<const float4*>(pos), tri, H, W, static_cast<const unsigned long long*>(vis),

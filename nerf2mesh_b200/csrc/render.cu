@@ -174,8 +174,8 @@ int n2m_s0_render_rounds(const n2m_s0_params* p, const float* rays_o, const floa
         if (int e = check_launch("s0_render(plan)")) return e;
         k_r_march<<<div_up(N, 128u), 128, 0, st>>>(*p, rays_o, rays_d, bitfield, rays_t, rays_far, alive, N, ctl, static_cast<float4*>(recs));
         if (int e = check_launch("s0_render(march)")) return e;
-        if (int e = n2m_s0_encode_fwd(p, recs, ctl, Mcap, rays_o, rays_d, table, offsets, enc_tiles, nullptr, nullptr, stream)) return e;
-        if (int e = n2m_s0_mlp_fwd(p, enc_tiles, ctl, Mcap, wpack, out, nullptr, stream)) return e;
+        if (int e = n2m_s0_encode_fwd(p, recs, ctl, Mcap, rays_o, rays_d, table, offsets, enc_tiles, 0, 1, stream)) return e;
+        if (int e = n2m_s0_mlp_fwd(p, enc_tiles, ctl, Mcap, wpack, out, nullptr, 0, 1, stream)) return e;
         k_r_composite<<<div_up(N, 128u), 128, 0, st>>>(*p, static_cast<const float4*>(out), static_cast<const float4*>(recs), ctl, alive, N,
                                                       rays_t, weights_sum, depth, image);
         if (int e = check_launch("s0_render(composite)")) return e;

@@ -259,12 +259,6 @@ k_ssaa_down2(const uint8_t* __restrict__ feats, uint32_t h0, uint32_t w0, uint32
 
 using namespace n2m;
 
-static int texture_sms() {
-    static int n = 0;
-    if (!n) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev); if (n <= 0) n = 132; }
-    return n;
-}
-
 extern "C" {
 
 int n2m_s1_bake_points(const float* rast, const float* verts, const int32_t* tri, uint32_t W, uint32_t y0, uint32_t y1, uint32_t cap,
@@ -294,7 +288,7 @@ int n2m_s1_geo_feat(const void* enc_tiles, const int32_t* counters, uint32_t Pca
         if (e != cudaSuccess) return fail("s1_geo_feat(attribute)", cudaGetErrorString(e));
         attr = true;
     }
-    const uint32_t grid = min(Pcap / kTile, (uint32_t)(3 * texture_sms()));          // 67.6 KB of shared memory: 3 CTAs per SM
+    const uint32_t grid = min(Pcap / kTile, (uint32_t)(3 * num_sms()));          // 67.6 KB of shared memory: 3 CTAs per SM
     k_s1_geo_feat<<<grid, 128, G_BYTES, as_stream(stream)>>>(static_cast<const uint8_t*>(enc_tiles), counters, static_cast<const uint8_t*>(wpack),
                                                              pix, feats, feats_f32);
     return check_launch("s1_geo_feat");

@@ -36,7 +36,6 @@ PP = ctypes.POINTER(S0Params)
 _lib.register({
     "n2m_s0_init": [],
     "n2m_s0_set_serial_march": [I],
-    "n2m_s0_set_tv_mode": [I],
     "n2m_s0_tv": [PP, P, P, U, P, P, P, P, P, P, P],
     "n2m_s0_tv_random": [PP, P, P, P, P, P, U, P, P],
     "n2m_s0_pack_weights": [P, P, P],
@@ -44,28 +43,21 @@ _lib.register({
     "n2m_s0_unpack_tables": [P, P, U, P, P, P],
     "n2m_s0_unpack_grads": [P, U, P, P, P, P],
     "n2m_s0_march": [PP, P, P, P, P, P, P, U, P, P, P, P, U, P],
-    "n2m_s0_encode_fwd": [PP, P, P, U, P, P, P, P, P, P, P, P],
+    "n2m_s0_encode_fwd": [PP, P, P, U, P, P, P, P, P, U, U, P],
     "n2m_s0_encode_points": [PP, P, P, P, U, P, P, P, P],
     "n2m_s0_grid_points": [U, U, U, F, P, P, P],
     "n2m_s0_grid_update": [P, U, F, P, P],
     "n2m_s0_packbits_dev": [P, U, P, F, P, P],
-    "n2m_s0_mlp_fwd": [PP, P, P, U, P, P, P, P],
-    "n2m_s0_composite_loss": [PP, P, P, P, P, U, U, P, P, P, P, P, P, P, P, P],
-    "n2m_s0_mlp_bwd": [PP, P, P, P, U, P, P, P, P, P],
-    "n2m_s0_encode_bwd": [PP, P, P, U, P, P, P, P, P, P, P, P],
-    "n2m_s0_adam": [P, P, P, P, P, U, P, P, P, P, P, P, F, P],
-    "n2m_s0_encode_fwd_part": [PP, P, P, U, P, P, P, P, P, P, P, U, U, P],
-    "n2m_s0_mlp_fwd_part": [PP, P, P, U, P, P, P, U, U, P],
-    "n2m_s0_composite_loss_part": [PP, P, P, P, P, U, U, P, P, P, P, P, P, P, P, U, U, P],
-    "n2m_s0_mlp_bwd_part": [PP, P, P, P, U, P, P, P, P, U, U, P],
-    "n2m_s0_encode_bwd_part": [PP, P, P, U, P, P, P, P, P, P, P, U, U, P],
+    "n2m_s0_mlp_fwd": [PP, P, P, U, P, P, P, U, U, P],
+    "n2m_s0_composite_loss": [PP, P, P, P, P, U, U, P, P, P, P, P, P, P, P, U, U, P],
+    "n2m_s0_mlp_bwd": [PP, P, P, P, U, P, P, P, P, U, U, P],
+    "n2m_s0_encode_bwd": [PP, P, P, U, P, P, P, P, P, P, P, U, U, P],
     "n2m_s0_adam_head": [P, P, P],
     "n2m_s0_adam_tables": [P, P, P, P, P, U, P, F, P],
     "n2m_s0_adam_tables_keep": [P, P, P, P, P, U, P, F, P],
     "n2m_s0_adam_mlp": [P, P, P, P, P, P, F, P],
     "n2m_s0_adam_post": [P, P],
     "n2m_mark_untrained_grid": [P, U, P, U, P, F, P, F, U, U, P, P, P],
-    "n2m_s0_fused_init": [],
     "n2m_s0_fwd_fused": [PP, P, P, U, P, P, P, P, P, P, P, P, P],
     "n2m_s0_render_begin": [PP, P, P, P, P, U, P, P, P, P, P, P, P, P],
     "n2m_s0_render_rounds": [PP, P, P, P, U, P, U, P, P, P, P, P, P, P, U, P, P, P, P, P, P, P],
@@ -149,7 +141,6 @@ class Stage0Trainer:
         self.device = torch.device(device)
         dev = self.device
         call("n2m_s0_init")
-        call("n2m_s0_fused_init")
         c = cfg
         offs = level_offsets(3, c.num_levels, c.per_level_scale, c.base_resolution, c.log2_hashmap_size, False)
         self.offsets = torch.from_numpy(offs).to(dev)
@@ -193,17 +184,18 @@ class Stage0Trainer:
         self.dout = torch.zeros(Mc, 4, device=dev)
         self.image = torch.zeros(N, 3, device=dev); self.weights_sum = torch.zeros(N, device=dev); self.depth = torch.zeros(N, device=dev)
         self.loss_acc = torch.zeros(4, device=dev)          # [0] rgb(+mask) loss, [1] sum |spec|^2
+        # explicit-point evaluation (density-grid update, density volume): positions and their count
+        self._pts = torch.zeros(Mc, 3, device=dev)
+        self._pcount = torch.zeros(4, dtype=torch.int32, device=dev)
         self.params = S0Params()
         self._fill_params(shading_full=True, gt_has_alpha=True)
         self.fused_fwd = False              # True: gather + MLP forward as one warp-specialised launch (whole batch: needs nparts == 1)
         self.use_cam_near_far = False       # clamp (near, far) with the per-ray values in the slot's cam_nf (--enable_cam_near_far)
-        self._tv_overlap = True             # TV gradient as its own launch overlapped with the MLP kernels (tv mode 2)
-        self._tv_stream = None
+        self._tv_stream = None              # the TV launch runs on its own stream, overlapped with the MLP kernels
         self.nparts = 1                     # ray-range parts run as concurrent chains on forked streams (1, 2, 4 or 8)
         self._part_streams = []
         self._adam_stream = None
         self.tv_fallback_points = 1000000   # GridEncoder.grad_total_variation's random-point fallback (grid.py:172,181-183)
-        call("n2m_s0_set_tv_mode", 2 if self._tv_overlap else 0)
         # EMA of the parameters (Trainer(ema_decay=0.95), main.py:241): shadow buffers are allocated by enable_ema()
         self.ema_decay = None
         self.ema_num_updates = 0
@@ -252,21 +244,6 @@ class Stage0Trainer:
             raise ValueError("fused_bwd: the fused MLP-backward + scatter kernel was removed; the backward is k_mlp_bwd followed by "
                              "k_s0_encode_bwd")
 
-    @property
-    def tv_overlap(self):
-        return self._tv_overlap
-
-    @tv_overlap.setter
-    def tv_overlap(self, on):
-        """True: the TV gradient is its own launch (n2m_s0_tv) on a forked stream; False: it is evaluated inside the scatter kernel.
-        The kernel-side mode is a process-wide switch, so it is set here together with the host-side flag (and captured graphs of
-        the other mode are dropped)."""
-        on = bool(on)
-        if on != self._tv_overlap:
-            self._tv_overlap = on
-            call("n2m_s0_set_tv_mode", 2 if on else 0)
-            self._graphs = {k: g for k, g in self._graphs.items() if k[0] in ("march", "adam", "peer_adam")}
-
     # current slot's buffers under their historical names
     rays_o = property(lambda self: self.slots[self.cur].rays_o)
     rays_d = property(lambda self: self.slots[self.cur].rays_d)
@@ -290,6 +267,14 @@ class Stage0Trainer:
         p.contract, p.max_steps, p.cascades, p.grid_size = int(c.contract), c.max_steps, c.cascade, c.grid_size
         p.num_levels, p.base_res = c.num_levels, c.base_resolution
         p.shading_full, p.gt_has_alpha = int(shading_full), int(gt_has_alpha)
+
+    def params_with(self, **fields):
+        """A copy of `params` with `fields` overridden, e.g. params_with(shading_full=0) for sigma-only evaluation."""
+        p = S0Params()
+        ctypes.memmove(ctypes.byref(p), ctypes.byref(self.params), ctypes.sizeof(S0Params))
+        for name, value in fields.items():
+            setattr(p, name, value)
+        return p
 
     def reset_parameters(self, seed=0):
         """Reference initialisation: embeddings U(-1e-4, 1e-4) (grid.py:144-146), nn.Linear default
@@ -451,21 +436,20 @@ class Stage0Trainer:
              ptr(self.noises), self.N, ptr(self.rays), ptr(self.counters), ptr(self.tbuf), ptr(self.recs), self.Mcap, stream())
 
     def encode_fwd(self, part=0, nparts=1):
-        call("n2m_s0_encode_fwd_part", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
-             ptr(self.table), ptr(self.offsets), ptr(self.enc_tiles), ptr(self.gtables[self.parity]), ptr(self.opt_state),
-             part, nparts, stream())
+        call("n2m_s0_encode_fwd", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
+             ptr(self.table), ptr(self.offsets), ptr(self.enc_tiles), part, nparts, stream())
 
     def mlp_fwd(self, part=0, nparts=1):
-        call("n2m_s0_mlp_fwd_part", self._pp(), ptr(self.enc_tiles), ptr(self.counters), self.Mcap, ptr(self.wpack), ptr(self.out),
+        call("n2m_s0_mlp_fwd", self._pp(), ptr(self.enc_tiles), ptr(self.counters), self.Mcap, ptr(self.wpack), ptr(self.out),
              self.loss_acc.data_ptr() + 4, part, nparts, stream())
 
     def composite_loss(self, part=0, nparts=1):
-        call("n2m_s0_composite_loss_part", self._pp(), ptr(self.out), ptr(self.recs), ptr(self.rays), ptr(self.counters), self.N, self.Mcap,
+        call("n2m_s0_composite_loss", self._pp(), ptr(self.out), ptr(self.recs), ptr(self.rays), ptr(self.counters), self.N, self.Mcap,
              ptr(self.gt), ptr(self.bg), ptr(self.opt_state), ptr(self.dout), ptr(self.image), ptr(self.weights_sum), ptr(self.depth),
              ptr(self.loss_acc), part, nparts, stream())
 
     def mlp_bwd(self, part=0, nparts=1):
-        call("n2m_s0_mlp_bwd_part", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.Mcap, ptr(self.wpack),
+        call("n2m_s0_mlp_bwd", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.Mcap, ptr(self.wpack),
              ptr(self.denc_tiles), ptr(self.g_mlp), ptr(self.opt_state), part, nparts, stream())
 
     def fwd_fused(self):
@@ -473,7 +457,7 @@ class Stage0Trainer:
              ptr(self.table), ptr(self.offsets), ptr(self.wpack), ptr(self.enc_tiles), ptr(self.out), self.loss_acc.data_ptr() + 4, stream())
 
     def encode_bwd(self, part=0, nparts=1):
-        call("n2m_s0_encode_bwd_part", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
+        call("n2m_s0_encode_bwd", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
              ptr(self.denc_tiles), ptr(self.table), ptr(self.offsets), ptr(self.gtables[self.parity]), ptr(self.opt_state),
              part, nparts, stream())
 
@@ -511,7 +495,7 @@ class Stage0Trainer:
         call("n2m_s0_adam_post", ptr(self.opt_state), stream())
 
     def forward_backward(self):
-        """march -> encode -> MLP -> composite+loss -> MLP backward -> scatter(+TV); gradients stay in
+        """march -> encode (|| TV) -> MLP -> composite+loss -> MLP backward -> scatter; gradients stay in
         gtable / g_mlp (loss-scaled)."""
         self.march()
         self._compute()
@@ -523,14 +507,12 @@ class Stage0Trainer:
           gather -> MLP -> composite -> MLP backward -> scatter of every part runs on its own stream, so the
           latency-bound tensor-core MLP kernels of one part share the SMs with the memory-bound gather / scatter
           kernels of another.
-        * `tv_overlap`: the TV-gradient kernel (memory bound, independent of the MLPs) runs on a forked stream as well; otherwise it
-          is evaluated inside the scatter kernel and only the (normally empty) random-point fallback is launched behind it.
+        * with lambda_tv > 0 the TV-gradient kernel (memory bound, independent of the MLPs) runs on a forked stream as well.
         All forks are joined before returning (and they are graph-capturable: fork/join by events only)."""
         self.loss_acc.zero_()
         main = torch.cuda.current_stream()
         P_ = int(self.nparts)
-        has_tv = self.cfg.lambda_tv > 0
-        fork_tv = self.tv_overlap and has_tv
+        fork_tv = self.cfg.lambda_tv > 0
 
         def launch_tv():
             if fork_tv:
@@ -572,12 +554,10 @@ class Stage0Trainer:
                 main.wait_stream(st)
         if fork_tv:
             main.wait_stream(self._tv_stream)
-        elif has_tv:
-            self.tv_random()          # TV itself ran inside the scatter kernels (tv mode 0), which also counted the groups
 
-    def _compute_dp(self):
-        """`_compute` for the fused data-parallel optimizers: the gradient buffers of the OTHER parity (consumed by every peer in the
-        previous step's reduce, which ended with a barrier) are zeroed on a side stream underneath this step's forward / backward."""
+    def _under_zeroing(self, fn, zero_mlp=False):
+        """Run `fn` while the gradient table of the OTHER parity (and with `zero_mlp` its MLP gradient) is zeroed on a side stream
+        underneath; joined before returning."""
         main = torch.cuda.current_stream()
         if self._zero_stream is None:
             self._zero_stream = torch.cuda.Stream(device=self.device)
@@ -585,9 +565,15 @@ class Stage0Trainer:
         side.wait_stream(main)
         with torch.cuda.stream(side):
             self.gtables[self.parity ^ 1].zero_()
-            self.g_mlps[(self.parity ^ 1) % len(self.g_mlps)].zero_()
-        self._compute()
+            if zero_mlp:
+                self.g_mlps[(self.parity ^ 1) % len(self.g_mlps)].zero_()
+        fn()
         main.wait_stream(side)
+
+    def _compute_dp(self):
+        """`_compute` for the fused data-parallel optimizers: the gradient buffers of the OTHER parity (consumed by every peer in the
+        previous step's reduce, which ended with a barrier) are zeroed underneath this step's forward / backward."""
+        self._under_zeroing(self._compute, zero_mlp=True)
 
     def _compute_then_adam(self):
         """forward + backward + optimizer of one step (single GPU).  With `defer_zero` the gradient table the PREVIOUS step used is
@@ -596,38 +582,21 @@ class Stage0Trainer:
             self._compute()
             self.adam()
             return
-        main = torch.cuda.current_stream()
-        if self._zero_stream is None:
-            self._zero_stream = torch.cuda.Stream(device=self.device)
-        side = self._zero_stream
-        side.wait_stream(main)
-        with torch.cuda.stream(side):
-            self.gtables[self.parity ^ 1].zero_()
-        self._compute()
-        self.adam(keep_grads=True)
-        main.wait_stream(side)
+
+        def body():
+            self._compute()
+            self.adam(keep_grads=True)
+        self._under_zeroing(body)
 
     def _compute_sg(self):
         """`_compute` of a single-GPU step whose optimizer is launched separately (see `prefetch_at`)."""
         if not self.defer_zero:
             self._compute()
             return
-        main = torch.cuda.current_stream()
-        if self._zero_stream is None:
-            self._zero_stream = torch.cuda.Stream(device=self.device)
-        side = self._zero_stream
-        side.wait_stream(main)
-        with torch.cuda.stream(side):
-            self.gtables[self.parity ^ 1].zero_()
-        self._compute()
-        main.wait_stream(side)
+        self._under_zeroing(self._compute)
 
     def _adam_sg(self):
         self.adam(keep_grads=self.defer_zero)
-
-    def _step_body(self):
-        self.march()
-        self._compute_then_adam()
 
     # -------------------------------------------------------------------------------------------
     def _graph(self, name, fn):
@@ -639,7 +608,7 @@ class Stage0Trainer:
             key = (name, self.parity)
         else:
             key = (name, self.cur, self.parity, int(self.params.shading_full), int(self.params.gt_has_alpha), int(self.nparts),
-                   bool(self.tv_overlap), bool(self.fused_fwd), int(self.tv_fallback_points), bool(self.defer_zero))
+                   bool(self.fused_fwd), int(self.tv_fallback_points), bool(self.defer_zero))
         g = self._graphs.get(key)
         if g is None:
             g = torch.cuda.CUDAGraph()
@@ -771,13 +740,8 @@ class Stage0Trainer:
             if cells % W:
                 raise ValueError(f"grid cells ({cells}) not divisible by the world size ({W})")
         lo, hi = rank * (cells // W), (rank + 1) * (cells // W)
-        if not hasattr(self, "_pts"):
-            self._pts = torch.zeros(self.Mcap, 3, device=dev)
-            self._pcount = torch.zeros(4, dtype=torch.int32, device=dev)
-            self._pparams = S0Params()
-        ctypes.memmove(ctypes.byref(self._pparams), ctypes.byref(self.params), ctypes.sizeof(S0Params))
-        self._pparams.shading_full = 0                       # sigma only: skip the specular rounds
-        pp = ctypes.byref(self._pparams)
+        pparams = self.params_with(shading_full=0)           # sigma only: skip the specular rounds
+        pp = ctypes.byref(pparams)
         for cas in range(c.cascade):
             bound = float(min(2 ** cas, c.bound))
             row = self.density_grid[cas]
@@ -789,7 +753,7 @@ class Stage0Trainer:
                 call("n2m_s0_encode_points", pp, ptr(self._pts), None, ptr(self._pcount), self.Mcap, ptr(self.table),
                      ptr(self.offsets), ptr(self.enc_tiles), stream())
                 call("n2m_s0_mlp_fwd", pp, ptr(self.enc_tiles), ptr(self._pcount), self.Mcap, ptr(self.wpack), ptr(self.out),
-                     None, stream())
+                     None, 0, 1, stream())
                 call("n2m_s0_grid_update", ptr(self.out), cnt, float(decay), row.data_ptr() + 4 * first, stream())
             if W > 1:
                 dist.all_gather_into_tensor(row, row[lo:hi].clone(), group=shard_group)
@@ -817,12 +781,8 @@ class Stage0Trainer:
             return torch.nan_to_num(grid0, 0)
         mean = getattr(self, "mean_density", None)
         thresh = min(float(mean.item()), density_thresh) if mean is not None else density_thresh
-        if not hasattr(self, "_pcount"):
-            self._pcount = torch.zeros(4, dtype=torch.int32, device=dev)
-            self._pparams = S0Params()
-        ctypes.memmove(ctypes.byref(self._pparams), ctypes.byref(self.params), ctypes.sizeof(S0Params))
-        self._pparams.shading_full = 0
-        pp = ctypes.byref(self._pparams)
+        pparams = self.params_with(shading_full=0)
+        pp = ctypes.byref(pparams)
         lin = torch.linspace(-1, 1, R, device=dev)
         sig = torch.empty(R ** 3, device=dev)
         per = max(1, self.Mcap // (R * R))                # x-slabs per chunk
@@ -834,7 +794,8 @@ class Stage0Trainer:
             self._pcount.fill_(n)
             call("n2m_s0_encode_points", pp, ptr(pts), None, ptr(self._pcount), self.Mcap, ptr(self.table), ptr(self.offsets),
                  ptr(self.enc_tiles), stream())
-            call("n2m_s0_mlp_fwd", pp, ptr(self.enc_tiles), ptr(self._pcount), self.Mcap, ptr(self.wpack), ptr(self.out), None, stream())
+            call("n2m_s0_mlp_fwd", pp, ptr(self.enc_tiles), ptr(self._pcount), self.Mcap, ptr(self.wpack), ptr(self.out), None, 0, 1,
+                 stream())
             sig[x0 * R * R: x1 * R * R] = self.out[:n, 0]
         mask = torch.nn.functional.interpolate(grid0[None, None], size=[R] * 3, mode="nearest")[0, 0] > thresh
         return torch.nan_to_num(sig.view(R, R, R) * mask, 0)
@@ -869,9 +830,8 @@ class Stage0Trainer:
                 chunk=chunk, cap=cap, rays_t=torch.empty(chunk, device=dev), rays_far=torch.empty(chunk, device=dev),
                 alive=torch.empty(2 * chunk, dtype=torch.int32, device=dev), ctl=torch.zeros(16, dtype=torch.int32, device=dev),
                 recs=torch.empty(cap, 4, device=dev), enc=torch.empty(cap * 64, dtype=torch.float16, device=dev),
-                out=torch.empty(cap, 4, device=dev), params=S0Params())
-        ctypes.memmove(ctypes.byref(rb["params"]), ctypes.byref(self.params), ctypes.sizeof(S0Params))
-        rb["params"].shading_full = int(shading == "full")
+                out=torch.empty(cap, 4, device=dev))
+        rb["params"] = self.params_with(shading_full=int(shading == "full"))        # the parameter block of this call's launches
         pp = ctypes.byref(rb["params"])
         sched = (ctypes.c_uint32 * len(self.RENDER_SCHEDULE))(*self.RENDER_SCHEDULE)
         more = (ctypes.c_uint32 * 2)(512, 512)
@@ -953,8 +913,7 @@ class Stage0Trainer:
         self.denc_tiles = torch.zeros(Mc * 64, dtype=torch.float16, device=dev)
         self.out = torch.zeros(Mc, 4, device=dev)
         self.dout = torch.zeros(Mc, 4, device=dev)
-        if hasattr(self, "_pts"):
-            del self._pts
+        self._pts = torch.zeros(Mc, 3, device=dev)
         self._graphs = {}
 
     def drop_prefetch(self):

@@ -22,7 +22,6 @@ from . import _lib
 from ._lib import F, I, P, U, call, ptr, stream
 from . import raster as dr
 from . import texture  # noqa: F401  (the stage-1 export, texture.export_stage1; binds include/n2m_b200_texture.h)
-from .stage0 import S0Params
 
 _lib.register({
     "n2m_s1_points": [P, P, P, P, U, U, U, U, P, P, P, P, P, P],
@@ -82,10 +81,8 @@ class Stage1Trainer:
             self.vert_state = torch.zeros(4, device=dev)                  # [0] Adam step count of this group, [1] current lr_vert
             self.vert_scratch = torch.zeros(6 * V, device=dev)
             self.grad_offsets = torch.zeros(V, 3, device=dev)             # total gradient of the last step (diagnostic / tests)
-        self.params = S0Params()
-        ctypes.memmove(ctypes.byref(self.params), ctypes.byref(t0.params), ctypes.sizeof(S0Params))
-        self.params.lambda_specular = 0.0          # the specular regulariser is a stage-0 loss (utils.py:726,735-738)
-        self.params.lambda_tv = 0.0
+        # the specular regulariser and TV are stage-0 losses (utils.py:726,735-738)
+        self.params = t0.params_with(lambda_specular=0.0, lambda_tv=0.0)
 
     def _pp(self):
         return ctypes.byref(self.params)
@@ -102,7 +99,8 @@ class Stage1Trainer:
              ptr(self.counters), ptr(self.inv), ptr(self.pts), ptr(self.pdirs), ptr(self.recs), stream())
         call("n2m_s0_encode_points", self._pp(), ptr(self.pts), ptr(self.pdirs), ptr(self.counters), self.cap, ptr(t0.table),
              ptr(t0.offsets), ptr(self.enc_tiles), stream())
-        call("n2m_s0_mlp_fwd", self._pp(), ptr(self.enc_tiles), ptr(self.counters), self.cap, ptr(t0.wpack), ptr(self.out), None, stream())
+        call("n2m_s0_mlp_fwd", self._pp(), ptr(self.enc_tiles), ptr(self.counters), self.cap, ptr(t0.wpack), ptr(self.out), None, 0, 1,
+             stream())
         if self.antialias:
             n = self.h * self.w
             th = self.topology
@@ -126,9 +124,9 @@ class Stage1Trainer:
             call("n2m_s1_loss", ptr(self.out), ptr(self.inv), ptr(gt), gt.shape[-1], ptr(bg), self.h0, self.w0, self.ssaa, self.lambda_mask,
                  ptr(t0.opt_state), ptr(self.dout), ptr(self.image), ptr(self.weights_sum), ptr(self.loss_acc), stream())
         call("n2m_s0_mlp_bwd", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.cap, ptr(t0.wpack),
-             ptr(self.denc_tiles), ptr(t0.g_mlp), ptr(t0.opt_state), stream())
+             ptr(self.denc_tiles), ptr(t0.g_mlp), ptr(t0.opt_state), 0, 1, stream())
         call("n2m_s0_encode_bwd", self._pp(), ptr(self.recs), ptr(self.counters), self.cap, ptr(self.pts), ptr(self.pdirs),
-             ptr(self.denc_tiles), ptr(t0.table), ptr(t0.offsets), ptr(t0.gtables[t0.parity]), ptr(t0.opt_state), stream())
+             ptr(self.denc_tiles), ptr(t0.table), ptr(t0.offsets), ptr(t0.gtables[t0.parity]), ptr(t0.opt_state), 0, 1, stream())
 
     def step(self, mvp, rays_d, gt, bg, shading="full", lr=None, use_graph=False):
         """One optimizer step on one view: mvp [4,4], rays_d [h0*w0,3] (unnormalised), gt [h0*w0, 3 or 4], bg [h0*w0,3].

@@ -1,4 +1,4 @@
-"""Time the stand-alone MLP backward (n2m_s0_mlp_bwd_part, k_mlp_bwd) on bench.py's lego batch, against its bound from shapes.
+"""Time the stand-alone MLP backward (n2m_s0_mlp_bwd, k_mlp_bwd) on bench.py's lego batch, against its bound from shapes.
 
     python profiles/mlp_bwd_time.py [--iters 200] [--warmup 20] [--shading {full,diffuse}]
 

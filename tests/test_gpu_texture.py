@@ -15,7 +15,7 @@ from nerf2mesh_b200 import raster as dr
 from nerf2mesh_b200 import synthetic as S
 from nerf2mesh_b200 import texture as X
 from nerf2mesh_b200._lib import call, ptr, stream
-from nerf2mesh_b200.stage0 import S0Params, Stage0Config, Stage0Trainer
+from nerf2mesh_b200.stage0 import Stage0Config, Stage0Trainer
 
 pytestmark = pytest.mark.gpu
 
@@ -65,16 +65,15 @@ def test_geo_feat_is_bit_identical_to_the_forward_kernel(t0):
     baker.pts[:P] = pts
     baker.pix[:P] = torch.arange(P, dtype=torch.int32, device="cuda")
     baker.counters.zero_(); baker.counters[1] = P
-    params = S0Params()
-    ctypes.memmove(ctypes.byref(params), ctypes.byref(t0.params), ctypes.sizeof(S0Params))
-    params.shading_full = 0
+    params = t0.params_with(shading_full=0)
     call("n2m_s0_encode_points", ctypes.byref(params), ptr(baker.pts), None, ptr(baker.counters), baker.cap, ptr(t0.table), ptr(t0.offsets),
          ptr(baker.enc_tiles), stream())
     feats = torch.zeros(P, 6, dtype=torch.uint8, device="cuda")
     f32 = torch.full((baker.cap, 6), -1.0, device="cuda")
     call("n2m_s1_geo_feat", ptr(baker.enc_tiles), ptr(baker.counters), baker.cap, ptr(t0.wpack), ptr(baker.pix), ptr(feats), ptr(f32), stream())
     out = torch.zeros(baker.cap, 4, device="cuda")
-    call("n2m_s0_mlp_fwd", ctypes.byref(params), ptr(baker.enc_tiles), ptr(baker.counters), baker.cap, ptr(t0.wpack), ptr(out), None, stream())
+    call("n2m_s0_mlp_fwd", ctypes.byref(params), ptr(baker.enc_tiles), ptr(baker.counters), baker.cap, ptr(t0.wpack), ptr(out), None, 0, 1,
+         stream())
     torch.cuda.synchronize()
     assert torch.equal(f32[:P, :3], out[:P, 1:4])
     assert (f32[P:] == -1.0).all()                                     # rows past the count are not written

@@ -188,12 +188,12 @@ def test_step_orchestration_call_sequence_two_launch_backward(monkeypatch):
         setattr(tr, k, T())
     tr.gtables, tr.g_mlps, tr.defer_zero, tr._zero_stream = [T(), T()], [T()], False, None
     tr.params = S0.S0Params(); tr.Mcap, tr.N, tr.rows, tr.parity, tr.device = 128, 4, 160, 0, "cpu"
-    tr._tv_overlap, tr._tv_stream, tr._part_streams = True, None, []
+    tr._tv_stream, tr._part_streams = None, []
     tr._adam_stream = None
     tr.fused_fwd, tr.tv_fallback_points, tr._graphs = False, 1000, {}
 
     tv = ["n2m_s0_tv", "n2m_s0_tv_random"]
-    chain = ["n2m_s0_encode_fwd_part", "n2m_s0_mlp_fwd_part", "n2m_s0_composite_loss_part", "n2m_s0_mlp_bwd_part", "n2m_s0_encode_bwd_part"]
+    chain = ["n2m_s0_encode_fwd", "n2m_s0_mlp_fwd", "n2m_s0_composite_loss", "n2m_s0_mlp_bwd", "n2m_s0_encode_bwd"]
     adam = ["n2m_s0_adam_head", "n2m_s0_adam_mlp", "n2m_s0_adam_tables", "n2m_s0_adam_post"]
 
     def names():
@@ -202,12 +202,14 @@ def test_step_orchestration_call_sequence_two_launch_backward(monkeypatch):
     tr.nparts = 1
     tr._compute_then_adam()
     assert names() == [chain[0]] + tv + chain[1:] + adam
+    assert all(a[-3:-1] == (0, 1) for n, a in calls if n in chain)          # the whole batch is part 0 of 1
     for P_ in (2, 4):
         calls.clear(); tr.nparts = P_
         tr._compute_then_adam()
         assert names() == tv + chain * P_ + adam
-        parts = [a[-3:-1] for n, a in calls if n == "n2m_s0_mlp_bwd_part"]
-        assert parts == [(k, P_) for k in range(P_)]
+        for stage in chain:
+            parts = [a[-3:-1] for n, a in calls if n == stage]
+            assert parts == [(k, P_) for k in range(P_)]
     # the backward is always MLP backward, then scatter: the fused backward is gone, and asking for it fails
     import pytest
     with pytest.raises(ValueError):
@@ -222,22 +224,21 @@ def test_step_orchestration_call_sequence_two_launch_backward(monkeypatch):
     with pytest.raises(RuntimeError):
         tr._compute()
     tr.fused_fwd = False
-    # TV inside the scatter kernel (tv mode 0): no TV launch, the fallback probe follows the scatter
-    calls.clear(); tr.nparts = 1
-    tr.tv_overlap = False
-    assert names() == ["n2m_s0_set_tv_mode"]
-    calls.clear()
-    tr._compute_then_adam()
-    assert names() == chain + ["n2m_s0_tv_random"] + adam
     # deferred zeroing of the gradient table: same launches, the optimizer variant that leaves the rows alone
-    calls.clear(); tr.defer_zero = True
+    calls.clear(); tr.nparts = 1; tr.defer_zero = True
     tr._compute_then_adam()
-    assert names() == chain + ["n2m_s0_tv_random"] + adam[:2] + ["n2m_s0_adam_tables_keep", adam[3]]
+    assert names() == [chain[0]] + tv + chain[1:] + adam[:2] + ["n2m_s0_adam_tables_keep", adam[3]]
     tr.defer_zero = False
     # lambda_tv == 0: no TV work at all
     calls.clear(); tr.cfg.lambda_tv = 0.0
     tr._compute_then_adam()
     assert names() == chain + adam
+    # constructing a trainer sets kernel attributes and uploads its own parameters, and switches no process-wide mode that another
+    # trainer's launches would read
+    calls.clear()
+    monkeypatch.setattr(torch.cuda, "synchronize", lambda *a, **k: None)
+    S0.Stage0Trainer(S0.Stage0Config(num_rays=128, max_steps=16, log2_hashmap_size=10), device="cpu")
+    assert names() == ["n2m_s0_init", "n2m_s0_pack_tables", "n2m_s0_pack_weights"]
 
 
 def test_step_prefetch_ordering(monkeypatch):

@@ -72,6 +72,18 @@ int n2m_s1_loss_aa(const void* aa, const float* gt, uint32_t gt_channels, const 
                    n2m_stream_t stream);
 int n2m_s1_dout(const void* grad_rgba, const int32_t* inv, uint32_t num_pixels, void* dout, n2m_stream_t stream);
 
+/* mesh refinement (opt.refine: update_triangles_errors, renderer.py:893-903,923-943; utils.py:720-721): n2m_s1_loss_err and
+ * n2m_s1_loss_aa_err are n2m_s1_loss / n2m_s1_loss_aa that also, for every low-res pixel whose top-left super-sample (y0*ssaa, x0*ssaa)
+ * of rast [h,w,4] is covered by face f (rast.w = f + 1, f < F), add the pixel's loss (before the 1/(h0*w0) mean and without loss_scale)
+ * to face_err[f] and 1 to face_cnt[f].  face_err, face_cnt [F] f32 accumulate across calls (the caller zeroes them); fp32 atomics, so
+ * face_err is deterministic up to summation order and face_cnt is exact below 2^24 hits per face. */
+int n2m_s1_loss_err(const void* out, const int32_t* inv, const float* gt, uint32_t gt_channels, const float* bg, uint32_t h0, uint32_t w0,
+                    uint32_t ssaa, float lambda_mask, const float* loss_scale, void* dout, float* image, float* weights_sum, float* loss_out,
+                    const float* rast, float* face_err, float* face_cnt, uint32_t F, n2m_stream_t stream);
+int n2m_s1_loss_aa_err(const void* aa, const float* gt, uint32_t gt_channels, const float* bg, uint32_t h0, uint32_t w0, uint32_t ssaa,
+                       float lambda_mask, const float* loss_scale, void* d_aa, float* image, float* weights_sum, float* loss_out,
+                       const float* rast, float* face_err, float* face_cnt, uint32_t F, n2m_stream_t stream);
+
 /* vertex-offset optimizer of stage 1 (`vertices_offsets`: nn.Parameter at renderer.py:160, Adam group with lr_vert at :180; regularisers
  * utils.py:750-779).  n2m_s1_vert_check: non-finite scan of the loss-scaled clip-space gradient grad_vclip [V,4] into found_inf
  * (opt_state[3]) -- call it BEFORE the optimizer head.  n2m_s1_vert_step (between the optimizer head and its post kernel):

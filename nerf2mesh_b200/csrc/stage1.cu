@@ -18,6 +18,8 @@
 //   n2m_s1_loss_aa                    clamp, alphas * rgbs, ssaa average, background mix, loss; gradient w.r.t. the antialiased image
 //   n2m_antialias_backward            -> gradient w.r.t. the (r, g, b, mask) image and w.r.t. the clip-space vertices (vertices_offsets)
 //   n2m_s1_dout                       gather of the colour gradient back to the compacted points
+// With mesh refinement on (opt.refine), n2m_s1_loss_err / n2m_s1_loss_aa_err replace the two loss launches: the same kernels, which also
+// accumulate each pixel's loss and a hit into the face it sees (update_triangles_errors, renderer.py:893-903,923-943; utils.py:720-721).
 #include "n2m_common.cuh"
 #include "../../include/n2m_b200_raster.h"
 
@@ -72,11 +74,26 @@ __global__ void k_s1_finish_count(int32_t* __restrict__ counters, uint32_t cap) 
     counters[3] = 0;
 }
 
+// ERR (refinement on): face_err[f] += the pixel's loss before the 1/Q, face_cnt[f] += 1, for the face f seen at the pixel's top-left
+// super-sample (y0 * ssaa, x0 * ssaa) of rast -- update_triangles_errors (renderer.py:893-903,923-943): the nearest-neighbour minification
+// of trig_id picks that sample, and a pixel whose sample is background charges nothing.  The face id comes from rast, not from inv, so a
+// pixel whose point fell beyond the max_points cap still charges its face.
+__device__ __forceinline__ void s1_face_error(const float* __restrict__ rast, uint32_t y0, uint32_t x0, uint32_t w, uint32_t ssaa, float loss_q,
+                                              float* __restrict__ face_err, float* __restrict__ face_cnt, uint32_t F) {
+    const float id = rast[4 * ((size_t)(y0 * ssaa) * w + x0 * ssaa) + 3];
+    if (id > 0.f) {
+        const uint32_t f = (uint32_t)id - 1u;
+        if (f < F) { atomicAdd(face_err + f, loss_q); atomicAdd(face_cnt + f, 1.f); }
+    }
+}
+
 // one thread per low-resolution pixel
+template <bool ERR>
 __global__ void __launch_bounds__(256)
 k_s1_loss(const float4* __restrict__ out, const int32_t* __restrict__ inv, const float* __restrict__ gt, uint32_t gt_channels,
           const float* __restrict__ bg, uint32_t h0, uint32_t w0, uint32_t ssaa, float lambda_mask, const float* __restrict__ loss_scale,
-          float4* __restrict__ dout, float* __restrict__ image, float* __restrict__ weights_sum, float* __restrict__ loss_out) {
+          float4* __restrict__ dout, float* __restrict__ image, float* __restrict__ weights_sum, float* __restrict__ loss_out,
+          const float* __restrict__ rast, float* __restrict__ face_err, float* __restrict__ face_cnt, uint32_t F) {
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t Q = h0 * w0;
     float my_loss = 0.f;
@@ -116,6 +133,7 @@ k_s1_loss(const float4* __restrict__ out, const int32_t* __restrict__ inv, const
                 const int32_t k = inv[(size_t)(y0 * ssaa + dy) * w + x0 * ssaa + dx];
                 if (k >= 0) dout[k] = d;
             }
+        if constexpr (ERR) s1_face_error(rast, y0, x0, w, ssaa, my_loss, face_err, face_cnt, F);
         my_loss /= (float)Q;
     }
     // block reduction -> one atomic per block
@@ -150,11 +168,13 @@ k_s1_dout(const float4* __restrict__ grad_rgba, const int32_t* __restrict__ inv,
     if (k >= 0) { const float4 g = grad_rgba[i]; dout[k] = make_float4(0.f, g.x, g.y, g.z); }
 }
 
-// one thread per low-resolution pixel; aa [h*w] float4 = antialiased (r, g, b, alpha); d_aa = d loss / d aa * loss_scale
+// one thread per low-resolution pixel; aa [h*w] float4 = antialiased (r, g, b, alpha); d_aa = d loss / d aa * loss_scale; ERR as in k_s1_loss
+template <bool ERR>
 __global__ void __launch_bounds__(256)
 k_s1_loss_aa(const float4* __restrict__ aa, const float* __restrict__ gt, uint32_t gt_channels, const float* __restrict__ bg, uint32_t h0,
              uint32_t w0, uint32_t ssaa, float lambda_mask, const float* __restrict__ loss_scale, float4* __restrict__ d_aa,
-             float* __restrict__ image, float* __restrict__ weights_sum, float* __restrict__ loss_out) {
+             float* __restrict__ image, float* __restrict__ weights_sum, float* __restrict__ loss_out,
+             const float* __restrict__ rast, float* __restrict__ face_err, float* __restrict__ face_cnt, uint32_t F) {
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     const uint32_t Q = h0 * w0;
     float my_loss = 0.f;
@@ -204,6 +224,7 @@ k_s1_loss_aa(const float4* __restrict__ aa, const float* __restrict__ gt, uint32
                 d.w = (v.w >= 0.f && v.w <= 1.f) ? sc * (e0 * (cr - b0) + e1 * (cg - b1) + e2 * (cb - b2)) + dmask : 0.f;
                 d_aa[i] = d;
             }
+        if constexpr (ERR) s1_face_error(rast, y0, x0, w, ssaa, my_loss, face_err, face_cnt, F);
         my_loss /= (float)Q;
     }
 #pragma unroll
@@ -296,6 +317,34 @@ __global__ void k_s1_vert_tick(const float* __restrict__ st, float* __restrict__
     if (threadIdx.x == 0 && blockIdx.x == 0 && st[3] == 0.f) vst[0] += 1.f;
 }
 
+// the two entry points of each loss kernel: ERR = false (refinement off) and ERR = true (+ the per-face error scatter)
+template <bool ERR>
+int launch_s1_loss(const void* out, const int32_t* inv, const float* gt, uint32_t gt_channels, const float* bg, uint32_t h0, uint32_t w0,
+                   uint32_t ssaa, float lambda_mask, const float* loss_scale, void* dout, float* image, float* weights_sum, float* loss_out,
+                   const float* rast, float* face_err, float* face_cnt, uint32_t F, n2m_stream_t stream, const char* what) {
+    N2M_REQUIRE(out && inv && gt && bg && loss_scale && dout && image && weights_sum && loss_out, what, "null pointer");
+    N2M_REQUIRE(gt_channels == 3 || gt_channels == 4, what, "gt must have 3 or 4 channels");
+    N2M_REQUIRE(!ERR || (rast && face_err && face_cnt), what, "null pointer");
+    k_s1_loss<ERR><<<div_up(h0 * w0, 256u), 256, 0, as_stream(stream)>>>(static_cast<const float4*>(out), inv, gt, gt_channels, bg, h0, w0, ssaa,
+                                                                        lambda_mask, loss_scale, static_cast<float4*>(dout), image, weights_sum,
+                                                                        loss_out, rast, face_err, face_cnt, F);
+    return check_launch(what);
+}
+
+template <bool ERR>
+int launch_s1_loss_aa(const void* aa, const float* gt, uint32_t gt_channels, const float* bg, uint32_t h0, uint32_t w0, uint32_t ssaa,
+                      float lambda_mask, const float* loss_scale, void* d_aa, float* image, float* weights_sum, float* loss_out,
+                      const float* rast, float* face_err, float* face_cnt, uint32_t F, n2m_stream_t stream, const char* what) {
+    N2M_REQUIRE(aa && gt && bg && loss_scale && d_aa && image && weights_sum && loss_out, what, "null pointer");
+    N2M_REQUIRE(gt_channels == 3 || gt_channels == 4, what, "gt must have 3 or 4 channels");
+    N2M_REQUIRE(ssaa >= 1, what, "ssaa must be >= 1");
+    N2M_REQUIRE(!ERR || (rast && face_err && face_cnt), what, "null pointer");
+    k_s1_loss_aa<ERR><<<div_up(h0 * w0, 256u), 256, 0, as_stream(stream)>>>(static_cast<const float4*>(aa), gt, gt_channels, bg, h0, w0, ssaa,
+                                                                           lambda_mask, loss_scale, static_cast<float4*>(d_aa), image,
+                                                                           weights_sum, loss_out, rast, face_err, face_cnt, F);
+    return check_launch(what);
+}
+
 }  // namespace
 }  // namespace n2m
 
@@ -319,11 +368,15 @@ int n2m_s1_points(const float* rast, const float* verts, const int32_t* tri, con
 int n2m_s1_loss(const void* out, const int32_t* inv, const float* gt, uint32_t gt_channels, const float* bg, uint32_t h0, uint32_t w0,
                 uint32_t ssaa, float lambda_mask, const float* loss_scale, void* dout, float* image, float* weights_sum, float* loss_out,
                 n2m_stream_t stream) {
-    N2M_REQUIRE(out && inv && gt && bg && loss_scale && dout && image && weights_sum && loss_out, "s1_loss", "null pointer");
-    N2M_REQUIRE(gt_channels == 3 || gt_channels == 4, "s1_loss", "gt must have 3 or 4 channels");
-    k_s1_loss<<<div_up(h0 * w0, 256u), 256, 0, as_stream(stream)>>>(static_cast<const float4*>(out), inv, gt, gt_channels, bg, h0, w0, ssaa,
-                                                                   lambda_mask, loss_scale, static_cast<float4*>(dout), image, weights_sum, loss_out);
-    return check_launch("s1_loss");
+    return launch_s1_loss<false>(out, inv, gt, gt_channels, bg, h0, w0, ssaa, lambda_mask, loss_scale, dout, image, weights_sum, loss_out,
+                                 nullptr, nullptr, nullptr, 0, stream, "s1_loss");
+}
+
+int n2m_s1_loss_err(const void* out, const int32_t* inv, const float* gt, uint32_t gt_channels, const float* bg, uint32_t h0, uint32_t w0,
+                    uint32_t ssaa, float lambda_mask, const float* loss_scale, void* dout, float* image, float* weights_sum, float* loss_out,
+                    const float* rast, float* face_err, float* face_cnt, uint32_t F, n2m_stream_t stream) {
+    return launch_s1_loss<true>(out, inv, gt, gt_channels, bg, h0, w0, ssaa, lambda_mask, loss_scale, dout, image, weights_sum, loss_out,
+                                rast, face_err, face_cnt, F, stream, "s1_loss_err");
 }
 
 int n2m_s1_rgba(const void* out, const int32_t* inv, uint32_t num_pixels, void* rgba, n2m_stream_t stream) {
@@ -343,12 +396,15 @@ int n2m_s1_dout(const void* grad_rgba, const int32_t* inv, uint32_t num_pixels, 
 int n2m_s1_loss_aa(const void* aa, const float* gt, uint32_t gt_channels, const float* bg, uint32_t h0, uint32_t w0, uint32_t ssaa,
                    float lambda_mask, const float* loss_scale, void* d_aa, float* image, float* weights_sum, float* loss_out,
                    n2m_stream_t stream) {
-    N2M_REQUIRE(aa && gt && bg && loss_scale && d_aa && image && weights_sum && loss_out, "s1_loss_aa", "null pointer");
-    N2M_REQUIRE(gt_channels == 3 || gt_channels == 4, "s1_loss_aa", "gt must have 3 or 4 channels");
-    N2M_REQUIRE(ssaa >= 1, "s1_loss_aa", "ssaa must be >= 1");
-    k_s1_loss_aa<<<div_up(h0 * w0, 256u), 256, 0, as_stream(stream)>>>(static_cast<const float4*>(aa), gt, gt_channels, bg, h0, w0, ssaa, lambda_mask,
-                                                                      loss_scale, static_cast<float4*>(d_aa), image, weights_sum, loss_out);
-    return check_launch("s1_loss_aa");
+    return launch_s1_loss_aa<false>(aa, gt, gt_channels, bg, h0, w0, ssaa, lambda_mask, loss_scale, d_aa, image, weights_sum, loss_out,
+                                    nullptr, nullptr, nullptr, 0, stream, "s1_loss_aa");
+}
+
+int n2m_s1_loss_aa_err(const void* aa, const float* gt, uint32_t gt_channels, const float* bg, uint32_t h0, uint32_t w0, uint32_t ssaa,
+                       float lambda_mask, const float* loss_scale, void* d_aa, float* image, float* weights_sum, float* loss_out,
+                       const float* rast, float* face_err, float* face_cnt, uint32_t F, n2m_stream_t stream) {
+    return launch_s1_loss_aa<true>(aa, gt, gt_channels, bg, h0, w0, ssaa, lambda_mask, loss_scale, d_aa, image, weights_sum, loss_out,
+                                   rast, face_err, face_cnt, F, stream, "s1_loss_aa_err");
 }
 
 int n2m_s1_vert_check(const float* grad_vclip, uint32_t V, float* opt_state, n2m_stream_t stream) {

@@ -11,11 +11,16 @@ the model state (hash tables, MLP weights, optimizer moments, GradScaler state) 
 image-loss gradient w.r.t. the vertices in `vertex_gradient()` -- the quantity the reference's vertex optimizer consumes.
 `lr_vert > 0` also trains the vertex offsets as the reference's default stage 1 does (`vertices_offsets`, renderer.py:160,180: an Adam
 group with lr_vert; regularisers lambda_lap * laplacian_smooth_loss (uniform) + lambda_offsets * mean(sum(offsets^2)), utils.py:750-779).
-Not built: re-meshing (`refine_and_decimate`, CPU mesh libraries) and the pytorch3d regularisers that are off by
-default (lambda_normal, lambda_edgelen).
+`refine=True` adds the error-guided mesh refinement of the reference's stage 1 (opt.refine, main.py:129-136): every step also adds each
+low-res pixel's loss and a hit to the face that pixel sees (update_triangles_errors, renderer.py:893-903,923-943, fused into the loss
+kernels) in `face_errors` / `face_counts`; `refine_mask()` turns them into the decimate / refine face mask of refine_and_decimate
+(renderer.py:217-240), and after the caller re-meshes on the CPU (decimate_and_refine_mesh, pymeshlab) `replace_mesh()` restarts the step on
+the new mesh (renderer.py:287-292, utils.py:1209-1210).  Not built: the pytorch3d regularisers that are off by default (lambda_normal,
+lambda_edgelen), several cascade meshes and SDF mode's all-ones refinement mask.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -28,6 +33,8 @@ _lib.register({
     "n2m_s1_loss": [P, P, P, U, P, U, U, U, F, P, P, P, P, P, P],
     "n2m_s1_rgba": [P, P, U, P, P],
     "n2m_s1_loss_aa": [P, P, U, P, U, U, U, F, P, P, P, P, P, P],
+    "n2m_s1_loss_err": [P, P, P, U, P, U, U, U, F, P, P, P, P, P, P, P, P, U, P],
+    "n2m_s1_loss_aa_err": [P, P, U, P, U, U, U, F, P, P, P, P, P, P, P, P, U, P],
     "n2m_s1_dout": [P, P, U, P, P],
     "n2m_s1_vert_check": [P, U, P, P],
     "n2m_s1_vert_step": [P, P, P, U, P, P, P, P, P, P, P, U, F, F, F, F, P, P, P, P],
@@ -36,7 +43,7 @@ _lib.register({
 
 class Stage1Trainer:
     def __init__(self, t0, vertices, triangles, h0, w0, ssaa=2, max_points=None, lambda_mask=0.1, antialias=False, pos_gradient_boost=1.0,
-                 lr_vert=0.0, lambda_lap=0.001, lambda_offsets=0.1):
+                 lr_vert=0.0, lambda_lap=0.001, lambda_offsets=0.1, refine=False):
         assert ssaa in (1, 2), "the ssaa average equals the reference's bilinear down-scale only at factors 1 and 2"
         self.t0 = t0
         dev = t0.device
@@ -62,10 +69,8 @@ class Stage1Trainer:
         self.antialias = bool(antialias)
         self.pos_gradient_boost = float(pos_gradient_boost)
         if self.antialias:
-            self.topology = dr.TopologyHash(self.triangles)               # once per mesh
             self.rgba = torch.zeros(n, 4, device=dev); self.aa = torch.zeros(n, 4, device=dev)
             self.d_aa = torch.zeros(n, 4, device=dev); self.g_rgba = torch.zeros(n, 4, device=dev)
-            self.grad_vclip = torch.zeros(self.vertices.shape[0], 4, device=dev)
         self.vclip = None
         self.mvp = None
         self._graphs, self._warm = {}, False
@@ -74,15 +79,29 @@ class Stage1Trainer:
         if self.lr_vert > 0:
             if not self.antialias:
                 raise ValueError("the image loss reaches the vertices through dr.antialias only: lr_vert > 0 needs antialias=True")
-            V = self.vertices.shape[0]
+            self.vert_state = torch.zeros(4, device=dev)                  # [0] Adam step count of this group, [1] current lr_vert
+        self.refine = bool(refine)
+        self._mesh_buffers()
+        # the specular regulariser and TV are stage-0 losses (utils.py:726,735-738)
+        self.params = t0.params_with(lambda_specular=0.0, lambda_tv=0.0)
+
+    def _mesh_buffers(self):
+        """(re)allocate everything sized by the mesh, for self.vertices / self.triangles: the edge hash, the clip-space vertex gradient,
+        the vertex-offset group (base = vertices, zero offsets and moments) and the per-face error accumulators"""
+        dev = self.t0.device
+        V, Fn = self.vertices.shape[0], self.triangles.shape[0]
+        if self.antialias:
+            self.topology = dr.TopologyHash(self.triangles)               # once per mesh
+            self.grad_vclip = torch.zeros(V, 4, device=dev)
+        if self.lr_vert > 0:
             self.base_vertices = self.vertices.clone()
             self.offsets = torch.zeros(V, 3, device=dev)
             self.m_vert = torch.zeros(V, 3, device=dev); self.v_vert = torch.zeros(V, 3, device=dev)
-            self.vert_state = torch.zeros(4, device=dev)                  # [0] Adam step count of this group, [1] current lr_vert
             self.vert_scratch = torch.zeros(6 * V, device=dev)
             self.grad_offsets = torch.zeros(V, 3, device=dev)             # total gradient of the last step (diagnostic / tests)
-        # the specular regulariser and TV are stage-0 losses (utils.py:726,735-738)
-        self.params = t0.params_with(lambda_specular=0.0, lambda_tv=0.0)
+        if self.refine:
+            # triangles_errors / triangles_errors_cnt (renderer.py:163-164): summed per-pixel loss and pixel count per face
+            self.face_errors = torch.zeros(Fn, device=dev); self.face_counts = torch.zeros(Fn, device=dev)
 
     def _pp(self):
         return ctypes.byref(self.params)
@@ -111,18 +130,22 @@ class Stage1Trainer:
     def loss_backward(self, gt, bg):
         t0 = self.t0
         self.loss_acc.zero_()
+        # refinement: the same loss kernels also scatter each pixel's loss into the face it sees (utils.py:720-721)
+        err = (ptr(self.rast), ptr(self.face_errors), ptr(self.face_counts), self.triangles.shape[0]) if self.refine else ()
         if self.antialias:
             n = self.h * self.w
             th = self.topology
-            call("n2m_s1_loss_aa", ptr(self.aa), ptr(gt), gt.shape[-1], ptr(bg), self.h0, self.w0, self.ssaa, self.lambda_mask,
-                 ptr(t0.opt_state), ptr(self.d_aa), ptr(self.image), ptr(self.weights_sum), ptr(self.loss_acc), stream())
+            call("n2m_s1_loss_aa_err" if self.refine else "n2m_s1_loss_aa", ptr(self.aa), ptr(gt), gt.shape[-1], ptr(bg), self.h0, self.w0,
+                 self.ssaa, self.lambda_mask, ptr(t0.opt_state), ptr(self.d_aa), ptr(self.image), ptr(self.weights_sum), ptr(self.loss_acc),
+                 *err, stream())
             self.grad_vclip.zero_()
             call("n2m_antialias_backward", ptr(self.rgba), ptr(self.rast), ptr(self.vclip), ptr(self.triangles), ptr(th.keys), ptr(th.opp),
                  th.slots, self.h, self.w, 4, ptr(self.d_aa), self.pos_gradient_boost, ptr(self.g_rgba), ptr(self.grad_vclip), stream())
             call("n2m_s1_dout", ptr(self.g_rgba), ptr(self.inv), n, ptr(self.dout), stream())
         else:
-            call("n2m_s1_loss", ptr(self.out), ptr(self.inv), ptr(gt), gt.shape[-1], ptr(bg), self.h0, self.w0, self.ssaa, self.lambda_mask,
-                 ptr(t0.opt_state), ptr(self.dout), ptr(self.image), ptr(self.weights_sum), ptr(self.loss_acc), stream())
+            call("n2m_s1_loss_err" if self.refine else "n2m_s1_loss", ptr(self.out), ptr(self.inv), ptr(gt), gt.shape[-1], ptr(bg), self.h0,
+                 self.w0, self.ssaa, self.lambda_mask, ptr(t0.opt_state), ptr(self.dout), ptr(self.image), ptr(self.weights_sum),
+                 ptr(self.loss_acc), *err, stream())
         call("n2m_s0_mlp_bwd", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.cap, ptr(t0.wpack),
              ptr(self.denc_tiles), ptr(t0.g_mlp), ptr(t0.opt_state), 0, 1, stream())
         call("n2m_s0_encode_bwd", self._pp(), ptr(self.recs), ptr(self.counters), self.cap, ptr(self.pts), ptr(self.pdirs),
@@ -185,3 +208,79 @@ class Stage1Trainer:
 
     def read_loss(self):
         return float(self.loss_acc[0].item())
+
+    def refine_mask(self):
+        """refine_and_decimate's face mask (renderer.py:217-240, one mesh, not SDF): mean error per face seen since the last reset,
+        thresholds = the 90th / 50th percentiles over the seen faces (numpy's default 'linear' method in float32, as np.percentile computes
+        them for the float32 errors).  Returns (mask [F] float32: 2 = refine (error > 90th), 1 = decimate (error < 50th), 0 = keep or
+        unseen, (thresh_refine, thresh_decimate)).  ValueError when no face has been seen."""
+        if not self.refine:
+            raise RuntimeError("refine_mask: construct Stage1Trainer(refine=True)")
+        cnt = self.face_counts
+        seen = cnt > 0
+        errors = self.face_errors.clone()
+        errors[seen] = errors[seen] / cnt[seen]
+        vals = torch.sort(errors[seen]).values
+        if vals.numel() == 0:
+            raise ValueError("refine_mask: no face has been seen since the mesh was (re)set")
+        t_refine, t_decimate = _percentile_f32(vals, 90), _percentile_f32(vals, 50)
+        mask = torch.zeros_like(errors)
+        mask[(errors > t_refine) & seen] = 2
+        mask[(errors < t_decimate) & seen] = 1
+        return mask, (float(t_refine), float(t_decimate))
+
+    def replace_mesh(self, vertices, triangles, reset_optimizer=True):
+        """Restart the step on a new mesh (the tail of refine_and_decimate, renderer.py:287-292, and the new optimizer of utils.py:1209-1210):
+        vertices [V,3] float, triangles [F,3] integer.  The vertices become the base of zero vertex offsets with zero Adam state; everything
+        sized by the mesh is reallocated, the face errors restart from zero and the captured per-view graphs are dropped (they hold the old
+        buffers' addresses).  reset_optimizer: also zero the shared Stage0Trainer's Adam moments and step count in place (a fresh
+        torch.optim.Adam; its own captured graphs stay valid), keeping the GradScaler state as the reference keeps its scaler.  The
+        reference also restarts its LambdaLR here (utils.py:1211): the schedule is the caller's (`step(lr=...)`), so the caller restarts it."""
+        dev = self.t0.device
+        if not (torch.is_tensor(vertices) and torch.is_tensor(triangles)):
+            raise ValueError("replace_mesh: vertices and triangles must be tensors")
+        if vertices.dim() != 2 or vertices.shape[1] != 3 or not vertices.is_floating_point() or vertices.shape[0] == 0:
+            raise ValueError("replace_mesh: vertices must be a float tensor [V,3], V >= 1")
+        if triangles.dim() != 2 or triangles.shape[1] != 3 or triangles.dtype not in _INT_DTYPES or triangles.shape[0] == 0:
+            raise ValueError("replace_mesh: triangles must be an integer tensor [F,3], F >= 1")
+        V = int(vertices.shape[0])
+        if int(triangles.min()) < 0 or int(triangles.max()) >= V:
+            raise ValueError(f"replace_mesh: triangles index outside the vertices (0..{V - 1})")
+        if not bool(torch.isfinite(vertices).all()):
+            raise ValueError("replace_mesh: vertices must be finite")
+        self._graphs.clear()
+        self._warm = False
+        self.vertices = vertices.to(dev, torch.float32).contiguous()
+        self.triangles = triangles.to(dev, torch.int32).contiguous()
+        self.rast = self.vclip = self.mvp = None
+        if self.lr_vert > 0:
+            self.vert_state[0:1].zero_()
+        self._mesh_buffers()
+        if reset_optimizer:
+            t0 = self.t0
+            for buf in (t0.m_table, t0.v_table, t0.m_mlp, t0.v_mlp):
+                buf.zero_()
+            t0.opt_state[2:3].zero_()
+
+
+_INT_DTYPES = (torch.int8, torch.uint8, torch.int16, torch.int32, torch.int64)
+
+
+def _percentile_f32(sorted_vals, q):
+    """np.percentile(x, q) (method 'linear') of a float32 tensor x given sorted: numpy keeps the float32 dtype throughout -- q / 100,
+    the virtual index (n - 1) * q, its fraction and the two-sided lerp are all float32 operations."""
+    n = sorted_vals.numel()
+    qf = np.float32(q) / np.float32(100)
+    vi = np.float32(n - 1) * qf
+    if vi >= n - 1:                                       # past the last index: the maximum (numpy's index -1, gamma against -1)
+        lo = hi = n - 1
+        gamma = vi - np.float32(-1)
+    else:
+        lo = int(np.floor(vi)); hi = lo + 1
+        gamma = vi - np.float32(lo)
+    a, b = sorted_vals[lo], sorted_vals[hi]
+    t = torch.tensor(float(gamma), dtype=torch.float32, device=sorted_vals.device)
+    d = b - a
+    if gamma >= 0.5:
+        return b - d * (1 - t)
+    return a + d * t

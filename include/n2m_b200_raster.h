@@ -56,6 +56,12 @@ int n2m_antialias_backward(const float* color, const float* rast, const float* p
  *   averaged over the h0*w0 pixels into loss_out[0]; dout [cap] float4 = (0, dL/drgb) * loss_scale for the covered pixels. */
 int n2m_s1_points(const float* rast, const float* verts, const int32_t* tri, const float* rays_d, uint32_t h, uint32_t w, uint32_t ssaa,
                   uint32_t cap, int32_t* counters, int32_t* inv, float* pts, float* pdirs, void* recs, n2m_stream_t stream);
+/* n2m_s1_points_contract: n2m_s1_points with contract != 0 applying the L-inf contract() of renderer.py:25-32 to each interpolated point
+ * before it is stored (unbounded scenes, Stage0Config.contract; the texture bake's n2m_s1_bake_points uses the same expression); pdirs are
+ * unchanged.  contract = 0 is n2m_s1_points. */
+int n2m_s1_points_contract(const float* rast, const float* verts, const int32_t* tri, const float* rays_d, uint32_t h, uint32_t w,
+                           uint32_t ssaa, uint32_t cap, int32_t* counters, int32_t* inv, float* pts, float* pdirs, void* recs,
+                           uint32_t contract, n2m_stream_t stream);
 int n2m_s1_loss(const void* out, const int32_t* inv, const float* gt, uint32_t gt_channels, const float* bg, uint32_t h0, uint32_t w0,
                 uint32_t ssaa, float lambda_mask, const float* loss_scale, void* dout, float* image, float* weights_sum, float* loss_out,
                 n2m_stream_t stream);

@@ -46,6 +46,17 @@ inline int num_sms() {
 // ---- small device helpers ---------------------------------------------------------------------
 __device__ __forceinline__ float clampf(float x, float lo, float hi) { return fminf(hi, fmaxf(lo, x)); }
 
+// contract() of renderer.py:25-32 (L-inf, in place): where(mag <= 1, x, x * (2 - 1 / mag) / mag), each operation rounded as torch rounds
+// it.  The one definition of the stage-1 step (k_s1_points) and the texture bake (k_s1_bake_points).
+__device__ __forceinline__ void contract_linf(float p[3]) {
+    const float mag = fmaxf(fabsf(p[0]), fmaxf(fabsf(p[1]), fabsf(p[2])));
+    if (!(mag <= 1.f)) {
+        const float s = __fsub_rn(2.f, __fdiv_rn(1.f, mag));
+#pragma unroll
+        for (int a = 0; a < 3; ++a) p[a] = __fdiv_rn(__fmul_rn(p[a], s), mag);
+    }
+}
+
 // 11-bit -> 31-bit spread for 3D Morton codes (bit i of v lands at bit 3i).  Identical to the
 // reference's multiply-and-mask form (raymarching.cu:56-63) for every v < 2048 (checked
 // exhaustively in tests/test_host_logic.py); the reference documents coords in [0,128).

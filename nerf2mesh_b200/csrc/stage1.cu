@@ -5,7 +5,8 @@
 //   n2m_s1_points                     covered pixels -> surface points: attribute interpolation of the vertex positions (dr.interpolate,
 //                                     renderer.py:862), nearest-neighbour up-sampling of the view directions (:828-829), compaction
 //                                     (xyzs[mask_flatten], :875-877) -- one kernel, no boolean-mask host sync; writes the march-record
-//                                     form (t = 0, origin = point) the stage-0 gather / backward kernels consume
+//                                     form (t = 0, origin = point) the stage-0 gather / backward kernels consume;
+//                                     n2m_s1_points_contract also applies contract() to the points (unbounded scenes, renderer.py:25-32)
 //   n2m_s0_encode_points, n2m_s0_mlp_fwd   self.rgb(x, d) (network.py:170-189) on tensor cores (sigma is computed and ignored)
 //   n2m_s1_loss                       alphas * rgbs, ssaa average (scale_img_hwc bilinear at factor 2 == 2x2 mean, :899-901), background
 //                                     mix (:907), MSE (+ mask) loss (utils.py:707-712) and its gradient w.r.t. every covered pixel's rgb
@@ -26,6 +27,9 @@
 namespace n2m {
 namespace {
 
+// CONTRACT (Stage0Config.contract): the interpolated point goes through contract() (n2m_common.cuh) before it is stored, as the reference
+// contracts xyzs before querying the colour field in an unbounded scene; the view directions are unchanged
+template <bool CONTRACT>
 __global__ void __launch_bounds__(256)
 k_s1_points(const float4* __restrict__ rast, const float* __restrict__ verts, const int32_t* __restrict__ tri,
             const float* __restrict__ rays_d, uint32_t h, uint32_t w, uint32_t ssaa, uint32_t cap, int32_t* __restrict__ counters,
@@ -54,10 +58,23 @@ k_s1_points(const float4* __restrict__ rast, const float* __restrict__ verts, co
             const float u = r.x, v = r.y, ww = 1.f - r.x - r.y;
             const uint32_t y = i / w, x = i % w;
             const uint32_t q = (y / ssaa) * (w / ssaa) + x / ssaa;            // nearest-neighbour source pixel of the low-res direction
+            if constexpr (CONTRACT) {
+                float p[3];
 #pragma unroll
-            for (int a = 0; a < 3; ++a) {
-                pts[3 * (size_t)k + a] = u * __ldg(verts + 3 * (size_t)i0 + a) + v * __ldg(verts + 3 * (size_t)i1 + a) + ww * __ldg(verts + 3 * (size_t)i2 + a);
-                pdirs[3 * (size_t)k + a] = __ldg(rays_d + 3 * (size_t)q + a);
+                for (int a = 0; a < 3; ++a)
+                    p[a] = u * __ldg(verts + 3 * (size_t)i0 + a) + v * __ldg(verts + 3 * (size_t)i1 + a) + ww * __ldg(verts + 3 * (size_t)i2 + a);
+                contract_linf(p);
+#pragma unroll
+                for (int a = 0; a < 3; ++a) {
+                    pts[3 * (size_t)k + a] = p[a];
+                    pdirs[3 * (size_t)k + a] = __ldg(rays_d + 3 * (size_t)q + a);
+                }
+            } else {
+#pragma unroll
+                for (int a = 0; a < 3; ++a) {
+                    pts[3 * (size_t)k + a] = u * __ldg(verts + 3 * (size_t)i0 + a) + v * __ldg(verts + 3 * (size_t)i1 + a) + ww * __ldg(verts + 3 * (size_t)i2 + a);
+                    pdirs[3 * (size_t)k + a] = __ldg(rays_d + 3 * (size_t)q + a);
+                }
             }
             recs[k] = make_float4(0.f, 0.f, 0.f, __int_as_float((int)k));      // t = 0: the "sample" is its origin
         }
@@ -352,17 +369,24 @@ using namespace n2m;
 
 extern "C" {
 
-int n2m_s1_points(const float* rast, const float* verts, const int32_t* tri, const float* rays_d, uint32_t h, uint32_t w, uint32_t ssaa,
-                  uint32_t cap, int32_t* counters, int32_t* inv, float* pts, float* pdirs, void* recs, n2m_stream_t stream) {
+int n2m_s1_points_contract(const float* rast, const float* verts, const int32_t* tri, const float* rays_d, uint32_t h, uint32_t w,
+                           uint32_t ssaa, uint32_t cap, int32_t* counters, int32_t* inv, float* pts, float* pdirs, void* recs,
+                           uint32_t contract, n2m_stream_t stream) {
     N2M_REQUIRE(rast && verts && tri && rays_d && counters && inv && pts && pdirs && recs, "s1_points", "null pointer");
     N2M_REQUIRE(ssaa >= 1 && h % ssaa == 0 && w % ssaa == 0 && h > 0 && w > 0, "s1_points", "resolution must be a multiple of ssaa");
     cudaStream_t st = as_stream(stream);
     cudaMemsetAsync(counters, 0, 4 * sizeof(int32_t), st);
-    k_s1_points<<<div_up(h * w, 256u), 256, 0, st>>>(reinterpret_cast<const float4*>(rast), verts, tri, rays_d, h, w, ssaa, cap, counters, inv,
-                                                   pts, pdirs, static_cast<float4*>(recs));
+    auto kernel = contract ? k_s1_points<true> : k_s1_points<false>;
+    kernel<<<div_up(h * w, 256u), 256, 0, st>>>(reinterpret_cast<const float4*>(rast), verts, tri, rays_d, h, w, ssaa, cap, counters, inv,
+                                               pts, pdirs, static_cast<float4*>(recs));
     if (int e = check_launch("s1_points")) return e;
     k_s1_finish_count<<<1, 32, 0, st>>>(counters, cap);
     return check_launch("s1_points(count)");
+}
+
+int n2m_s1_points(const float* rast, const float* verts, const int32_t* tri, const float* rays_d, uint32_t h, uint32_t w, uint32_t ssaa,
+                  uint32_t cap, int32_t* counters, int32_t* inv, float* pts, float* pdirs, void* recs, n2m_stream_t stream) {
+    return n2m_s1_points_contract(rast, verts, tri, rays_d, h, w, ssaa, cap, counters, inv, pts, pdirs, recs, 0, stream);
 }
 
 int n2m_s1_loss(const void* out, const int32_t* inv, const float* gt, uint32_t gt_channels, const float* bg, uint32_t h0, uint32_t w0,

@@ -44,14 +44,7 @@ k_s1_bake_points(const float4* __restrict__ rast, const float* __restrict__ vert
 #pragma unroll
     for (int a = 0; a < 3; ++a)
         p[a] = u * __ldg(verts + (size_t)i0 * 3 + a) + vv * __ldg(verts + (size_t)i1 * 3 + a) + w * __ldg(verts + (size_t)i2 * 3 + a);
-    if (contract) {         // contract() of renderer.py:25-32: where(mag <= 1, x, x * (2 - 1 / mag) / mag)
-        const float mag = fmaxf(fabsf(p[0]), fmaxf(fabsf(p[1]), fabsf(p[2])));
-        if (!(mag <= 1.f)) {
-            const float s = __fsub_rn(2.f, __fdiv_rn(1.f, mag));
-#pragma unroll
-            for (int a = 0; a < 3; ++a) p[a] = __fdiv_rn(__fmul_rn(p[a], s), mag);
-        }
-    }
+    if (contract) contract_linf(p);         // contract() of renderer.py:25-32 (n2m_common.cuh)
     pix[k] = (int32_t)i;
 #pragma unroll
     for (int a = 0; a < 3; ++a) pts[3 * (size_t)k + a] = p[a];

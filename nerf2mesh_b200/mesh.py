@@ -9,7 +9,14 @@ third-party CPU library) with the kernels of csrc/mcubes.cu (C ABI include/n2m_b
 `export_stage0_mesh(trainer, path, resolution)` is the reference's export up to (not including) its CPU clean-up / decimation:
 density volume (Stage0Trainer.density_volume == renderer.py:480-524) -> marching cubes -> `vertices / (resolution - 1) * 2 - 1` (:531) ->
 `mesh_0.ply`.  No CPU fallback: the volume must live on a CUDA device.
+
+Unbounded scenes (bound > 1, C = 1 + ceil(log2(bound)) cascades) also get one mesh per outer cascade (csrc/cascade.cu):
+`export_outer_meshes(trainer, path, env_reso)` is the non-SDF branch of export_stage0 for cas = 1 .. C-1 (renderer.py:606-672) up to its CPU
+clean-up / decimation -- occupancy volume of density_grid[cas] -> marching cubes at 0.5 -> world coordinates (float64, rounded once) ->
+removal of the centre box and of what lies outside the training AABB -> `mesh_{cas}.ply`.  `mark_unseen_triangles` is the reference's
+visibility test on those meshes, `load_stage0_meshes` picks every cascade's mesh up again for stage 1.
 """
+import ctypes
 import os
 import struct
 
@@ -18,11 +25,19 @@ import torch
 
 from . import _lib
 from . import mc_table
+from . import raster as dr
 from ._lib import F, P, U, call, ptr, stream
+
+D = ctypes.c_double
 
 _lib.register({
     "n2m_mc_count": [P, U, U, U, F, P, P, P, P],
     "n2m_mc_emit": [P, U, U, U, F, P, P, P, P, P, P, P],
+    "n2m_outer_occupancy": [P, U, U, F, P, P],
+    "n2m_outer_select": [P, U, U, D, D, D, D, D, D, D, P, P, P],
+    "n2m_rsv_count": [P, U, P, U, P, P, P],
+    "n2m_rsv_emit": [P, U, P, U, P, P, P, P, P, P, P],
+    "n2m_mark_seen_faces": [P, U, U, P, P],
 })
 
 _tables = {}
@@ -91,7 +106,8 @@ def read_ply(path):
 def export_stage0_mesh(trainer, save_path, resolution=512, density_thresh=10.0):
     """NeRFRenderer.export_stage0 for the inner region up to its CPU post-processing (renderer.py:471-531,543-544): density volume ->
     marching cubes at min(mean_density, density_thresh) -> world coordinates -> `<save_path>/mesh_0.ply`.  Returns (vertices, triangles)
-    on the device.  Cleaning / decimation (clean_mesh, decimate_mesh: pymeshlab) and the outer-region meshes stay the reference's code."""
+    on the device.  Cleaning / decimation (clean_mesh, decimate_mesh: pymeshlab) stay the caller's CPU code; the outer-region meshes of an
+    unbounded scene come from `export_outer_meshes`."""
     vol = trainer.density_volume(resolution=resolution, density_thresh=density_thresh)
     mean = getattr(trainer, "mean_density", None)
     thresh = min(float(mean.item()), density_thresh) if mean is not None else density_thresh
@@ -100,3 +116,124 @@ def export_stage0_mesh(trainer, save_path, resolution=512, density_thresh=10.0):
     os.makedirs(save_path, exist_ok=True)
     write_ply(os.path.join(save_path, "mesh_0.ply"), v, f)
     return v, f
+
+
+# ---- outer cascades of an unbounded scene ---------------------------------------------------------------------------------------------
+def _mesh_threshold(trainer, density_thresh):
+    mean = getattr(trainer, "mean_density", None)
+    return min(float(mean.item()), density_thresh) if mean is not None else density_thresh
+
+
+def outer_occupancy(grid, grid_size, resolution, thresh):
+    """grid [H^3] float32 CUDA (one cascade of the density grid, Morton order) -> float32 [R,R,R] 0/1 volume (x-major) =
+    nan_to_num(F.interpolate(occ[None,None], [R]*3, mode='trilinear')[0,0], 0) > thresh, occ the grid re-mapped to [H,H,H]
+    (renderer.py:618-628)"""
+    H, R = int(grid_size), int(resolution)
+    if not grid.is_cuda or grid.dtype != torch.float32 or grid.numel() != H ** 3:
+        raise ValueError(f"outer_occupancy: grid must be a float32 CUDA tensor of {H}^3 cells")
+    grid = grid.contiguous()
+    vol = torch.empty(R, R, R, device=grid.device)
+    call("n2m_outer_occupancy", ptr(grid), H, R, float(thresh), ptr(vol), stream())
+    return vol
+
+
+def outer_select(vertices, resolution, scale, box):
+    """vertices [V,3] float32 CUDA in index coordinates -> (world [V,3] float32, removed [V] bool): p = idx / (R-1) * 2 - 1, world = p * scale
+    in float64 rounded once; removed where every |p_c| <= 0.45 (renderer.py:633-635) or where world is outside the open box
+    box = (xmn, ymn, zmn, xmx, ymx, zmx) (:640-649)"""
+    V = int(vertices.shape[0])
+    vertices = vertices.float().contiguous()
+    out = torch.empty(V, 3, device=vertices.device)
+    removed = torch.empty(V, dtype=torch.uint8, device=vertices.device)
+    call("n2m_outer_select", ptr(vertices), V, int(resolution), float(scale), *(float(b) for b in box), ptr(out), ptr(removed), stream())
+    return out, removed.bool()
+
+
+def remove_selected_vertices(vertices, triangles, removed):
+    """pymeshlab's remove_selected_verts (meshutils.py:122-144) on the device: vertices [V,3] float32, triangles [F,3] int32, removed [V] bool
+    (CUDA) -> the unflagged vertices in their order (also those no face references any more) and the faces none of whose corners is flagged,
+    re-indexed."""
+    dev = vertices.device
+    vertices = vertices.float().contiguous(); triangles = triangles.int().contiguous()
+    V, Fn = int(vertices.shape[0]), int(triangles.shape[0])
+    removed = removed.to(dev, torch.uint8).contiguous()
+    if removed.numel() != V:
+        raise ValueError("remove_selected_vertices: one flag per vertex")
+    vkeep = torch.empty(V, dtype=torch.uint8, device=dev); fkeep = torch.empty(Fn, dtype=torch.uint8, device=dev)
+    call("n2m_rsv_count", ptr(removed), V, ptr(triangles), Fn, ptr(vkeep), ptr(fkeep), stream())
+    vinc = torch.cumsum(vkeep, 0, dtype=torch.int32); finc = torch.cumsum(fkeep, 0, dtype=torch.int32)
+    nv = int(vinc[-1].item()) if V else 0
+    nf = int(finc[-1].item()) if Fn else 0                                   # the host read-backs (output sizes)
+    voff = vinc - vkeep.to(torch.int32); foff = finc - fkeep.to(torch.int32)
+    out_v = torch.empty(nv, 3, device=dev); out_f = torch.empty(nf, 3, dtype=torch.int32, device=dev)
+    call("n2m_rsv_emit", ptr(vertices), V, ptr(triangles), Fn, ptr(vkeep), ptr(fkeep), ptr(voff), ptr(foff), ptr(out_v) if nv else None,
+         ptr(out_f) if nf else None, stream())
+    return out_v, out_f
+
+
+@torch.no_grad()
+def export_outer_meshes(trainer, save_path, env_reso=256, density_thresh=10.0):
+    """export_stage0's outer meshes (non-SDF, renderer.py:606-672) up to their CPU post-processing, for every cascade cas = 1 .. C-1:
+    occupancy volume of density_grid[cas] at env_reso^3 -> marching cubes at 0.5 -> (idx / (R-1) * 2 - 1) * (bound - half) with
+    bound = min(2^cas, cfg.bound), half = bound / R -> removal of the centre box and of the region outside the trainer's AABB shrunk by
+    half -> `<save_path>/mesh_{cas}.ply`.  Returns {cas: (vertices [V,3] float32, triangles [F,3] int32)} on the device; a cascade left
+    without vertices writes no file and is not in the dict.  The caller's CPU code then cleans and decimates each mesh (clean_mesh,
+    decimate_mesh with decimate_target // 2) and may drop the faces no training view sees (mark_unseen_triangles + remove_masked_trigs)."""
+    if hasattr(trainer, "drop_prefetch"):
+        trainer.drop_prefetch()
+    c = trainer.cfg
+    R, H = int(env_reso), int(c.grid_size)
+    thresh = _mesh_threshold(trainer, density_thresh)
+    xmn, ymn, zmn, xmx, ymx, zmx = trainer.aabb.detach().cpu().numpy().astype(np.float64).tolist()
+    os.makedirs(save_path, exist_ok=True)
+    meshes = {}
+    for cas in range(1, c.cascade):
+        bound = min(2 ** cas, c.bound)
+        half = bound / R
+        vol = outer_occupancy(trainer.density_grid[cas], H, R, thresh)
+        v, f = marching_cubes(vol, 0.5)
+        del vol
+        if v.shape[0] == 0:
+            continue
+        v, removed = outer_select(v, R, bound - half, (xmn + half, ymn + half, zmn + half, xmx - half, ymx - half, zmx - half))
+        v, f = remove_selected_vertices(v, f, removed)
+        if v.shape[0] == 0:
+            continue
+        write_ply(os.path.join(save_path, f"mesh_{cas}.ply"), v, f)
+        meshes[cas] = (v, f)
+    return meshes
+
+
+@torch.no_grad()
+def mark_unseen_triangles(vertices, triangles, mvps, H, W, glctx=None):
+    """The reference's visibility test (mark_unseen_triangles, renderer.py:947-981): rasterise the mesh in every view (mvps [B,4,4]) at
+    (H, W) and return the [F] bool mask of the faces no view covers.  As in the reference, an uncovered pixel's face index -1 marks the
+    last face, so face F-1 counts as seen whenever a view has an empty pixel."""
+    dev = torch.device("cuda", torch.cuda.current_device()) if not torch.is_tensor(vertices) or not vertices.is_cuda else vertices.device
+    v = torch.as_tensor(vertices).to(dev, torch.float32).contiguous()
+    tri = torch.as_tensor(triangles).to(dev, torch.int32).contiguous()
+    Fn = int(tri.shape[0])
+    seen = torch.zeros(Fn, dtype=torch.uint8, device=dev)
+    glctx = glctx or dr.RasterizeCudaContext(dev)
+    vh = torch.nn.functional.pad(v, pad=(0, 1), mode="constant", value=1.0)
+    for mvp in mvps:
+        vclip = torch.matmul(vh, torch.transpose(torch.as_tensor(mvp).to(dev, torch.float32), 0, 1)).float()
+        rast, _ = dr.rasterize(glctx, vclip[None], tri, (int(H), int(W)))
+        call("n2m_mark_seen_faces", ptr(rast), int(H) * int(W), Fn, ptr(seen), stream())
+    return seen == 0
+
+
+def load_stage0_meshes(mesh_dir, cascade):
+    """Per-cascade (vertices, triangles) lists for Stage1Trainer, as the reference's stage 1 loads them (renderer.py:130-157):
+    `mesh_{cas}_updated.ply` (written after a refinement) when it exists, else `mesh_{cas}.ply`.  float32 / int32 CPU tensors.
+    FileNotFoundError naming the file when a cascade has neither."""
+    vertices, triangles = [], []
+    for cas in range(int(cascade)):
+        path = os.path.join(mesh_dir, f"mesh_{cas}_updated.ply")
+        if not os.path.exists(path):
+            path = os.path.join(mesh_dir, f"mesh_{cas}.ply")
+            if not os.path.exists(path):
+                raise FileNotFoundError(f"load_stage0_meshes: no mesh for cascade {cas}: {path} does not exist")
+        v, f = read_ply(path)
+        vertices.append(torch.from_numpy(v).float()); triangles.append(torch.from_numpy(f.astype(np.int32)))
+    return vertices, triangles

@@ -15,8 +15,14 @@ group with lr_vert; regularisers lambda_lap * laplacian_smooth_loss (uniform) + 
 low-res pixel's loss and a hit to the face that pixel sees (update_triangles_errors, renderer.py:893-903,923-943, fused into the loss
 kernels) in `face_errors` / `face_counts`; `refine_mask()` turns them into the decimate / refine face mask of refine_and_decimate
 (renderer.py:217-240), and after the caller re-meshes on the CPU (decimate_and_refine_mesh, pymeshlab) `replace_mesh()` restarts the step on
-the new mesh (renderer.py:287-292, utils.py:1209-1210).  Not built: the pytorch3d regularisers that are off by default (lambda_normal,
-lambda_edgelen), several cascade meshes and SDF mode's all-ones refinement mask.
+the new mesh (renderer.py:287-292, utils.py:1209-1210).
+
+Unbounded scenes (bound > 1): `vertices` / `triangles` may be equal-length lists of per-cascade meshes (mesh.load_stage0_meshes), which the
+trainer concatenates with index offsets as the reference does (renderer.py:130-157, `v_cumsum` / `f_cumsum`); every kernel of the step then
+runs on the concatenated mesh, and `cascade_mesh(cas)` returns one cascade for the export.  Refinement looks at cascade 0 only
+(renderer.py:223-225) and `replace_mesh` replaces cascade 0, rebasing the outer cascades on their current vertices (:258-285).  With
+Stage0Config(contract=True) the surface points are contracted before the colour field is queried (n2m_s1_points_contract).  Not built: the
+pytorch3d regularisers that are off by default (lambda_normal, lambda_edgelen) and SDF mode's all-ones refinement mask.
 """
 import ctypes
 
@@ -30,6 +36,7 @@ from . import texture  # noqa: F401  (the stage-1 export, texture.export_stage1;
 
 _lib.register({
     "n2m_s1_points": [P, P, P, P, U, U, U, U, P, P, P, P, P, P],
+    "n2m_s1_points_contract": [P, P, P, P, U, U, U, U, P, P, P, P, P, U, P],
     "n2m_s1_loss": [P, P, P, U, P, U, U, U, F, P, P, P, P, P, P],
     "n2m_s1_rgba": [P, P, U, P, P],
     "n2m_s1_loss_aa": [P, P, U, P, U, U, U, F, P, P, P, P, P, P],
@@ -42,13 +49,15 @@ _lib.register({
 
 
 class Stage1Trainer:
+    v_cumsum = f_cumsum = ()            # per-cascade vertex / face offsets, set by _set_cascades
+
     def __init__(self, t0, vertices, triangles, h0, w0, ssaa=2, max_points=None, lambda_mask=0.1, antialias=False, pos_gradient_boost=1.0,
                  lr_vert=0.0, lambda_lap=0.001, lambda_offsets=0.1, refine=False):
         assert ssaa in (1, 2), "the ssaa average equals the reference's bilinear down-scale only at factors 1 and 2"
         self.t0 = t0
         dev = t0.device
-        self.vertices = vertices.to(dev, torch.float32).contiguous()
-        self.triangles = triangles.to(dev, torch.int32).contiguous()
+        self._set_cascades(*_cascade_lists(vertices, triangles))
+        self.contract = bool(getattr(t0.cfg, "contract", False))
         self.h0, self.w0, self.ssaa = int(h0), int(w0), int(ssaa)
         self.h, self.w = self.h0 * ssaa, self.w0 * ssaa
         n = self.h * self.w
@@ -85,6 +94,31 @@ class Stage1Trainer:
         # the specular regulariser and TV are stage-0 losses (utils.py:726,735-738)
         self.params = t0.params_with(lambda_specular=0.0, lambda_tv=0.0)
 
+    def _set_cascades(self, vertices, triangles):
+        """the concatenated mesh of the per-cascade lists: faces offset by the vertices of the cascades before them; v_cumsum / f_cumsum
+        (host ints) delimit cascade c as vertices[v_cumsum[c]:v_cumsum[c+1]], triangles[f_cumsum[c]:f_cumsum[c+1]].  No face links two
+        cascades, so the edge hash of the antialias / Laplacian kernels never does either: both act on each cascade on its own."""
+        dev = self.t0.device
+        self.v_cumsum, self.f_cumsum = [0], [0]
+        vs, fs = [], []
+        for v, f in zip(vertices, triangles):
+            off = self.v_cumsum[-1]
+            vs.append(v.to(dev, torch.float32)); fs.append(f.to(dev, torch.int32) + off if off else f.to(dev, torch.int32))
+            self.v_cumsum.append(self.v_cumsum[-1] + int(v.shape[0])); self.f_cumsum.append(self.f_cumsum[-1] + int(f.shape[0]))
+        self.vertices = (vs[0] if len(vs) == 1 else torch.cat(vs)).contiguous()
+        self.triangles = (fs[0] if len(fs) == 1 else torch.cat(fs)).contiguous()
+
+    @property
+    def cascades(self):
+        return len(self.v_cumsum) - 1
+
+    def cascade_mesh(self, cas):
+        """(vertices [Vc,3], triangles [Fc,3]) of cascade `cas` as it is now (base + offsets), triangles indexing its own vertices: the mesh the
+        export bakes and the one a refinement writes back as mesh_{cas}_updated.ply"""
+        v0, v1 = self.v_cumsum[cas], self.v_cumsum[cas + 1]
+        f0, f1 = self.f_cumsum[cas], self.f_cumsum[cas + 1]
+        return self.vertices[v0:v1], self.triangles[f0:f1] - v0
+
     def _mesh_buffers(self):
         """(re)allocate everything sized by the mesh, for self.vertices / self.triangles: the edge hash, the clip-space vertex gradient,
         the vertex-offset group (base = vertices, zero offsets and moments) and the per-face error accumulators"""
@@ -114,8 +148,12 @@ class Stage1Trainer:
         vclip = (torch.nn.functional.pad(self.vertices, (0, 1), value=1.0) @ mvp.T).contiguous()           # renderer.py:858
         self.vclip, self.mvp = vclip, mvp
         self.rast, _ = dr.rasterize(self.glctx, vclip[None], self.triangles, (self.h, self.w))
-        call("n2m_s1_points", ptr(self.rast), ptr(self.vertices), ptr(self.triangles), ptr(rays_d), self.h, self.w, self.ssaa, self.cap,
-             ptr(self.counters), ptr(self.inv), ptr(self.pts), ptr(self.pdirs), ptr(self.recs), stream())
+        pts_args = (ptr(self.rast), ptr(self.vertices), ptr(self.triangles), ptr(rays_d), self.h, self.w, self.ssaa, self.cap, ptr(self.counters),
+                    ptr(self.inv), ptr(self.pts), ptr(self.pdirs), ptr(self.recs))
+        if self.contract:               # the colour field of an unbounded scene is queried at contract(x) (renderer.py:25-32)
+            call("n2m_s1_points_contract", *pts_args, 1, stream())
+        else:
+            call("n2m_s1_points", *pts_args, stream())
         call("n2m_s0_encode_points", self._pp(), ptr(self.pts), ptr(self.pdirs), ptr(self.counters), self.cap, ptr(t0.table),
              ptr(t0.offsets), ptr(self.enc_tiles), stream())
         call("n2m_s0_mlp_fwd", self._pp(), ptr(self.enc_tiles), ptr(self.counters), self.cap, ptr(t0.wpack), ptr(self.out), None, 0, 1,
@@ -210,15 +248,17 @@ class Stage1Trainer:
         return float(self.loss_acc[0].item())
 
     def refine_mask(self):
-        """refine_and_decimate's face mask (renderer.py:217-240, one mesh, not SDF): mean error per face seen since the last reset,
-        thresholds = the 90th / 50th percentiles over the seen faces (numpy's default 'linear' method in float32, as np.percentile computes
-        them for the float32 errors).  Returns (mask [F] float32: 2 = refine (error > 90th), 1 = decimate (error < 50th), 0 = keep or
-        unseen, (thresh_refine, thresh_decimate)).  ValueError when no face has been seen."""
+        """refine_and_decimate's face mask (renderer.py:217-240, not SDF) over the faces of cascade 0 (:223-225; with one mesh, all faces):
+        mean error per face seen since the last reset, thresholds = the 90th / 50th percentiles over the seen faces (numpy's default 'linear'
+        method in float32, as np.percentile computes them for the float32 errors).  Returns (mask [f_cumsum[1]] float32: 2 = refine
+        (error > 90th), 1 = decimate (error < 50th), 0 = keep or unseen, (thresh_refine, thresh_decimate)).  ValueError when no face of
+        cascade 0 has been seen."""
         if not self.refine:
             raise RuntimeError("refine_mask: construct Stage1Trainer(refine=True)")
-        cnt = self.face_counts
+        f1 = self.f_cumsum[1] if self.f_cumsum else None                  # None (no cascade bookkeeping): every face
+        cnt = self.face_counts[:f1]
         seen = cnt > 0
-        errors = self.face_errors.clone()
+        errors = self.face_errors[:f1].clone()
         errors[seen] = errors[seen] / cnt[seen]
         vals = torch.sort(errors[seen]).values
         if vals.numel() == 0:
@@ -235,8 +275,9 @@ class Stage1Trainer:
         sized by the mesh is reallocated, the face errors restart from zero and the captured per-view graphs are dropped (they hold the old
         buffers' addresses).  reset_optimizer: also zero the shared Stage0Trainer's Adam moments and step count in place (a fresh
         torch.optim.Adam; its own captured graphs stay valid), keeping the GradScaler state as the reference keeps its scaler.  The
-        reference also restarts its LambdaLR here (utils.py:1211): the schedule is the caller's (`step(lr=...)`), so the caller restarts it."""
-        dev = self.t0.device
+        reference also restarts its LambdaLR here (utils.py:1211): the schedule is the caller's (`step(lr=...)`), so the caller restarts it.
+        On a trainer of several cascades the new mesh replaces cascade 0 and every outer cascade takes its current vertices (base + offsets)
+        as its new base (renderer.py:258-285); v_cumsum / f_cumsum are rebuilt."""
         if not (torch.is_tensor(vertices) and torch.is_tensor(triangles)):
             raise ValueError("replace_mesh: vertices and triangles must be tensors")
         if vertices.dim() != 2 or vertices.shape[1] != 3 or not vertices.is_floating_point() or vertices.shape[0] == 0:
@@ -248,10 +289,10 @@ class Stage1Trainer:
             raise ValueError(f"replace_mesh: triangles index outside the vertices (0..{V - 1})")
         if not bool(torch.isfinite(vertices).all()):
             raise ValueError("replace_mesh: vertices must be finite")
+        outer = [self.cascade_mesh(cas) for cas in range(1, self.cascades)]
         self._graphs.clear()
         self._warm = False
-        self.vertices = vertices.to(dev, torch.float32).contiguous()
-        self.triangles = triangles.to(dev, torch.int32).contiguous()
+        self._set_cascades([vertices] + [v.clone() for v, _ in outer], [triangles] + [f for _, f in outer])
         self.rast = self.vclip = self.mvp = None
         if self.lr_vert > 0:
             self.vert_state[0:1].zero_()
@@ -264,6 +305,16 @@ class Stage1Trainer:
 
 
 _INT_DTYPES = (torch.int8, torch.uint8, torch.int16, torch.int32, torch.int64)
+
+
+def _cascade_lists(vertices, triangles):
+    """(vertices, triangles) as equal-length lists of per-cascade tensors: a single tensor is a list of one"""
+    if torch.is_tensor(vertices) and torch.is_tensor(triangles):
+        return [vertices], [triangles]
+    vertices, triangles = list(vertices), list(triangles)
+    if len(vertices) == 0 or len(vertices) != len(triangles):
+        raise ValueError("vertices and triangles: one tensor each, or equal-length non-empty lists of per-cascade tensors")
+    return vertices, triangles
 
 
 def _percentile_f32(sorted_vals, q):

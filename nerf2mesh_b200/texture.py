@@ -3,6 +3,7 @@ Host side of csrc/texture.cu (C ABI include/n2m_b200_texture.h).
 
     vt, ft = <xatlas UV unwrap of (vertices, triangles)>                  # CPU, the caller's (see INTEGRATION.md 3d)
     export_stage1(s1, save_path, vt, ft, resolution=4096)                 # -> mesh_0.obj, mesh_0.mtl, feat0_0.jpg, feat1_0.jpg, mlp.json
+    export_stage1(s1, save_path, [vt0, vt1, ...], [ft0, ft1, ...])       # several cascades: mesh_{cas}.obj ... per cascade, one mlp.json
 
 The stages, each callable on its own:
     uv_features(t0, vertices, triangles, vt, ft, h, w)  UV raster (n2m_rasterize of (vt * 2 - 1, 0, 1) / ft), positions interpolated with
@@ -222,16 +223,38 @@ def write_textures(save_path, feat0, feat1, cas=0):
             raise RuntimeError(f"cv2.imwrite failed for {name}")
 
 
+def texture_sizes(resolution, cascades):
+    """the texture size of each cascade (renderer.py:441-452): halved after a cascade while it is > 2048 -- 4096 gives 4096, 2048, 2048, ..."""
+    sizes, r = [], int(resolution)
+    for _ in range(int(cascades)):
+        sizes.append(r)
+        if r > 2048:
+            r //= 2
+    return sizes
+
+
 def export_stage1(s1, save_path, vt, ft, resolution=4096, band_rows=None):
-    """NeRFRenderer.export_stage1 for one mesh (cascade 0) from a Stage1Trainer: vertices (base + offsets), triangles, the model of its
-    Stage0Trainer (call t0.ema_apply() first to export the EMA parameters), the trainer's ssaa; vt [Nt,2] / ft [F,3] from the caller's UV
-    unwrap.  Writes mesh_0.obj, mesh_0.mtl, feat0_0.jpg, feat1_0.jpg, mlp.json under save_path; returns (feat0, feat1) on the device."""
+    """NeRFRenderer.export_stage1 from a Stage1Trainer (renderer.py:298-468): for every cascade `cas` of the trainer, its mesh
+    (s1.cascade_mesh(cas): vertices = base + offsets), the model of its Stage0Trainer (call t0.ema_apply() first to export the EMA
+    parameters) and the trainer's ssaa give mesh_{cas}.obj, mesh_{cas}.mtl, feat0_{cas}.jpg, feat1_{cas}.jpg under save_path; then mlp.json
+    with `cascade` = the number of cascades.  vt [Nt,2] / ft [F,3] come from the caller's UV unwrap of the mesh (of contract(vertices) when
+    cfg.contract, renderer.py:314); a trainer of several cascades takes lists vt[cas] / ft[cas], one unwrap per cascade.  The texture is
+    `resolution` for cascade 0 and halves after each cascade while it is > 2048 (texture_sizes).  Returns (feat0, feat1) on the device for
+    one mesh, the list of them per cascade for lists."""
     t0 = s1.t0
+    C = s1.cascades
+    per_cascade = isinstance(vt, (list, tuple))
+    vts, fts = (list(vt), list(ft)) if per_cascade else ([vt], [ft])
+    if len(vts) != C or len(fts) != C:
+        raise ValueError(f"export_stage1: the trainer has {C} cascade meshes: pass one (vt, ft) per cascade, as lists")
     os.makedirs(save_path, exist_ok=True)
-    h0 = w0 = int(resolution)
-    feat0, feat1 = bake_features(t0, s1.vertices, s1.triangles, vt, ft, h0, w0, ssaa=s1.ssaa, band_rows=band_rows)
-    write_textures(save_path, feat0, feat1)
-    write_obj(os.path.join(save_path, "mesh_0.obj"), s1.vertices, s1.triangles, vt, ft)
-    write_mtl(os.path.join(save_path, "mesh_0.mtl"))
-    write_mlp_json(os.path.join(save_path, "mlp.json"), specular_weights(t0), bound=t0.cfg.bound, cascade=1)
-    return feat0, feat1
+    feats = []
+    for cas, size in enumerate(texture_sizes(resolution, C)):
+        v, f = s1.cascade_mesh(cas)
+        feat0, feat1 = bake_features(t0, v, f, vts[cas], fts[cas], size, size, ssaa=s1.ssaa, band_rows=band_rows)
+        write_textures(save_path, feat0, feat1, cas)
+        write_obj(os.path.join(save_path, f"mesh_{cas}.obj"), v, f, vts[cas], fts[cas], mtl_name=f"mesh_{cas}.mtl")
+        write_mtl(os.path.join(save_path, f"mesh_{cas}.mtl"), texture=f"feat0_{cas}.jpg")
+        feats.append((feat0, feat1))
+    write_mlp_json(os.path.join(save_path, "mlp.json"), specular_weights(t0), bound=t0.cfg.bound, cascade=C)
+    return feats if per_cascade else feats[0]

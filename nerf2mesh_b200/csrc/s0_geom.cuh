@@ -1,6 +1,9 @@
 // s0_geom.cuh -- sample / lattice geometry shared by the gather, scatter and fused kernels of the stage-0 train path
 // (stage0.cu, fused.cu): tile-image constants, the interleaved table entry, sample reconstruction from a march record, hash /
 // dense corner indices and trilinear weights of one level (gridencoder.cu:50-84,88-196 of the reference, same expressions).
+// Everything here is per level, so a kernel may visit the levels of a sample in any order or split them over launches / work items:
+// the scatter and TV passes of stage0.cu visit one level group of a tile at a time, so that the REDs of the CTAs running together
+// stay inside one group's slice of the gradient table (8 MiB per hashed level) instead of the whole 97.6 MB, twice the H100's L2.
 #pragma once
 #include "n2m_common.cuh"
 #include "../../include/n2m_b200_fused.h"

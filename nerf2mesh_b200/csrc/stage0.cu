@@ -2,6 +2,8 @@
 //   march (near/far + count + scan + sample records), hash-grid encode forward into tensor-core
 //   tile images, composite + loss + composite-backward per ray, hash-grid scatter (+TV) backward,
 //   table (de)interleave helpers.  The MLP stages live in mlp_tc.cu, the optimizer in optim.cu.
+//   The scatter and the TV pass walk the hash grid level group by level group rather than sample by sample: their RED target,
+//   the 97.6 MB gradient table, is twice the H100's L2, one group's slice of it fits (see "Level-group walk" below).
 #include "march_core.cuh"
 #include "s0_geom.cuh"
 #include <cstdlib>
@@ -177,7 +179,7 @@ k_s0_scan(int32_t* __restrict__ rays, uint32_t N, uint32_t Mcap, int32_t* __rest
         counters[0] = (int32_t)M;
         counters[1] = (int32_t)min(M, Mcap);
         counters[2] = M > Mcap ? 1 : 0;
-        counters[3] = 0;                 // samples inside the unit cube   } counted by this step's n2m_s0_tv (k_s0_encode_bwd<false, true, false>),
+        counters[3] = 0;                 // samples inside the unit cube   } counted by this step's n2m_s0_tv (k_s0_encode_bwd<false, true>),
         counters[15] = 0;                // samples outside the unit cube  } read by k_s0_tv_random (grid.py:181-183 fallback)
         // persistent capacity accounting (never reset by the march): steps that overflowed the sample slab, largest M seen
         if (M > Mcap) counters[13] += 1;
@@ -274,14 +276,49 @@ __device__ __forceinline__ float tv_grad(const TableEntry* __restrict__ tab, con
 // consecutive samples of a ray (= consecutive lanes) sit in the same lattice cell -- the 8 corner
 // contributions are first summed across each run of same-cell lanes with a segmented warp scan and only the
 // last lane of a run issues the red.global.add.v4.f32.  Fine levels (every lane its own cell) go straight to the atomics.
+//
+// Level-group walk.  The RED target is the whole gradient table: 6.1 M float4 rows = 97.6 MB at the default config (16 levels,
+// 2^19 rows per hashed level), twice the H100's 50 MB L2.  A thread that walks all 16 levels of its sample sends its REDs anywhere
+// in those 97.6 MB, so most of them miss L2 and cost a sector fill plus a write-back.  The work items of a launch are therefore
+// (level group, tile) pairs, ordered group-major and walked by a grid-stride loop: the CTAs resident at any moment work on
+// consecutive items, i.e. inside one or two groups, and the REDs land in one group's slice of the table (the dense levels 0-4
+// together, 13 MB; then one hashed level, 8 MiB, at a time).  The price is that every group re-reads the sample's march record
+// and the tile-image chunks that hold its own gradient columns -- small, L2-resident streams next to the RED traffic.  No result
+// depends on the order in which the items run: every item adds its own contributions and the TV sample counts are taken once,
+// by the items of group 0.
 // ------------------------------------------------------------------------------------------------
+constexpr uint32_t kDenseGroupLevels = 5;         // levels 0-4: 13 MB of gradient rows together at the default config
+constexpr uint32_t kHashedGroupLevels = 1;        // every later level its own group (two per group: slower step on the H100)
+constexpr uint32_t kLevelGroups = 1 + (kLevels - kDenseGroupLevels + kHashedGroupLevels - 1) / kHashedGroupLevels;
+
+__device__ __forceinline__ uint32_t group_first_level(uint32_t grp) {
+    return grp == 0 ? 0u : min(kLevels, kDenseGroupLevels + (grp - 1) * kHashedGroupLevels);
+}
+
+// The scatter's REDs carry an L2 evict-last hint: the lines of the current group's slice then outlast the streamed reads (march
+// records, tile images, the parameter table) between two REDs to the same sector.
+__device__ __forceinline__ uint64_t l2_evict_last() {
+    uint64_t pol;
+    asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ void red_add_v4(float4* dst, float a, float b, float c, uint64_t pol) {
+    asm volatile("red.global.add.L2::cache_hint.v4.f32 [%0], {%1, %2, %3, %4}, %5;"
+                 :: "l"(dst), "f"(a), "f"(b), "f"(c), "f"(0.f), "l"(pol) : "memory");
+}
+
+// one fp16 gradient column of a tile-image row (`row` = the row's first byte in chunk 0)
+__device__ __forceinline__ float denc_col(const uint8_t* row, uint32_t col) {
+    return __half2float(__ldg(reinterpret_cast<const __half*>(row + (col >> 3) * kChunkBytes + (col & 7) * 2)));
+}
+
 template <bool SCATTER, bool TV>
 __device__ __forceinline__ void
-encode_bwd_tile(const n2m_s0_params& p, const float4* __restrict__ recs,
-                const float* __restrict__ rays_o, const float* __restrict__ rays_d,
-                const uint8_t* __restrict__ denc_tiles, const TableEntry* __restrict__ table,
-                const int32_t* __restrict__ offsets, float4* __restrict__ gtable, float* __restrict__ loss_scale,
-                const PartRange pr, uint32_t tile, int32_t* tv_counts = nullptr) {
+encode_bwd_visit(const n2m_s0_params& p, const float4* __restrict__ recs,
+                 const float* __restrict__ rays_o, const float* __restrict__ rays_d,
+                 const uint8_t* __restrict__ denc_tiles, const TableEntry* __restrict__ table,
+                 const int32_t* __restrict__ offsets, float4* __restrict__ gtable, float* __restrict__ loss_scale,
+                 const PartRange pr, uint32_t tile, uint32_t l0, uint32_t l1, int32_t* tv_counts) {
     static_assert(SCATTER != TV, "a launch either scatters the feature gradients or evaluates TV");
     const uint32_t r = threadIdx.x;
     const uint32_t lane = r & 31;
@@ -295,26 +332,9 @@ encode_bwd_tile(const n2m_s0_params& p, const float4* __restrict__ recs,
         s.x = s.y = s.z = s.u = s.v = s.w = 0.5f; s.dx = s.dy = s.dz = 0.f;
     }
 
-    // this row's gradients: cols 3..18 density, 19..50 colour  (chunks 0..6)
+    // this row's gradients: cols 3..18 density, 19..50 colour (chunks 0..6); a group reads the columns of its own levels only
     const uint8_t* img = denc_tiles + (size_t)tile * kTileBytes + r * 16;
-    float g[56];
-#pragma unroll
-    for (uint32_t ch = 0; ch < 7; ++ch) {
-        uint4 q = make_uint4(0, 0, 0, 0);
-        if (SCATTER && active) q = *reinterpret_cast<const uint4*>(img + ch * kChunkBytes);
-        const uint32_t qq[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&qq[i]));
-            g[8 * ch + 2 * i] = f.x; g[8 * ch + 2 * i + 1] = f.y;
-        }
-    }
-    {   // fp16 overflow of the loss-scaled gradients => GradScaler semantics: flag, step is skipped
-        bool bad = false;
-#pragma unroll
-        for (int i = (int)kColDens; i < (int)kColDir; ++i) bad |= !isfinite(g[i]);
-        if (SCATTER && bad) loss_scale[3] = 1.f;
-    }
+    bool bad = false;          // fp16 overflow of the loss-scaled gradients => GradScaler semantics: flag, step is skipped
     // TV weight: lambda inside the unit cube, 10 lambda outside when bound > 1 (utils.py:815-821); w = weight / (2 D),
     // kept in the loss-scaled domain
     float tvw_lane = 0.f;
@@ -323,23 +343,28 @@ encode_bwd_tile(const n2m_s0_params& p, const float4* __restrict__ recs,
         const bool outer = p.grid_bound > 1 && mag > 1;
         const float lam = outer ? p.lambda_tv * 10 : p.lambda_tv;
         tvw_lane = active ? lam / 6 * loss_scale[0] : 0.f;
-        // how many samples each of the reference's TV calls would receive (utils.py:815-823: xyzs_inner / xyzs_outer, or all of them)
+        // how many samples each of the reference's TV calls would receive (utils.py:815-823: xyzs_inner / xyzs_outer, or all of
+        // them): counted once per sample, by the visit of the first level group
         const bool mine = j >= pr.lo && j < pr.hi;
         const uint32_t m_out = __ballot_sync(0xffffffffu, mine && outer), m_in = __ballot_sync(0xffffffffu, mine && !outer);
-        if (lane == 0 && tv_counts) {
+        if (lane == 0 && l0 == 0) {
             if (m_in) atomicAdd(tv_counts + 3, (int)__popc(m_in));
             if (m_out) atomicAdd(tv_counts + 15, (int)__popc(m_out));
         }
     }
 #pragma unroll 1
-    for (uint32_t l = 0; l < kLevels; ++l) {
+    for (uint32_t l = l0; l < l1; ++l) {
         const LevelGeom lg = level_geom(offsets, l, p.S, p.base_res);
         Corners c; uint32_t base[3]; bool hashed; uint32_t left[3];
         corners_of(lg, s.u, s.v, s.w, c, base, hashed, TV ? left : nullptr);
         float tvw = tvw_lane;
         float4* gt = gtable + lg.row0;
-        const float gd = active ? g[kColDens + l] : 0.f;
-        const float g0 = active ? g[kColColor + 2 * l] : 0.f, g1 = active ? g[kColColor + 2 * l + 1] : 0.f;
+        float gd = 0.f, g0 = 0.f, g1 = 0.f;
+        if (SCATTER && active) {
+            gd = denc_col(img, kColDens + l);
+            g0 = denc_col(img, kColColor + 2 * l); g1 = denc_col(img, kColColor + 2 * l + 1);
+            bad |= !isfinite(gd) || !isfinite(g0) || !isfinite(g1);
+        }
         float vd[8], v0[8], v1[8];
 #pragma unroll
         for (int k = 0; k < 8; ++k) { vd[k] = c.w[k] * gd; v0[k] = c.w[k] * g0; v1[k] = c.w[k] * g1; }
@@ -375,16 +400,19 @@ encode_bwd_tile(const n2m_s0_params& p, const float4* __restrict__ recs,
         if (issue) {
             if (SCATTER) {
 #pragma unroll
-                for (int k = 0; k < 8; ++k) atomicAdd(gt + c.row[k], make_float4(vd[k], v0[k], v1[k], 0.f));
+                const uint64_t pol = l2_evict_last();
+#pragma unroll
+                for (int k = 0; k < 8; ++k) red_add_v4(gt + c.row[k], vd[k], v0[k], v1[k], pol);
             }
             if (TV) atomicAdd(&gt[c.row[0]].x, tv_grad(table + lg.row0, c, base, left, lg.res, tvw));
         }
     }
+    if (SCATTER && bad) loss_scale[3] = 1.f;
 }
 
-// LOOP = false: the grid covers every tile of the slab (whole-batch launch), one tile per block, straight-line code
-// (faster than the looping form); LOOP = true: grid-stride over the part's tiles.
-template <bool SCATTER, bool TV, bool LOOP>
+// grid-stride over the (level group, tile) items of the part's range [lo, hi), group-major (see "Level-group walk" above); the
+// host sizes the grid to the CTAs that fit on the device at once
+template <bool SCATTER, bool TV>
 __global__ void __launch_bounds__(kTile)
 k_s0_encode_bwd(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* __restrict__ counters,
                 const float* __restrict__ rays_o, const float* __restrict__ rays_d,
@@ -393,17 +421,13 @@ k_s0_encode_bwd(n2m_s0_params p, const float4* __restrict__ recs, const int32_t*
                 uint32_t part, uint32_t nparts) {
     const PartRange pr = part_range(counters, part, nparts);
     if (pr.hi <= pr.lo) return;
-    const uint32_t t1 = (pr.hi + kTile - 1) / kTile;
-    if (!LOOP) {
-        const uint32_t tile = pr.lo / kTile + blockIdx.x;
-        if (tile < t1) encode_bwd_tile<SCATTER, TV>(p, recs, rays_o, rays_d, denc_tiles, table, offsets, gtable, loss_scale, pr, tile,
-                                                     const_cast<int32_t*>(counters));
-        return;
-    }
+    const uint32_t t0 = pr.lo / kTile, nt = (pr.hi + kTile - 1) / kTile - t0;
 #pragma unroll 1
-    for (uint32_t tile = pr.lo / kTile + blockIdx.x; tile < t1; tile += gridDim.x)
-        encode_bwd_tile<SCATTER, TV>(p, recs, rays_o, rays_d, denc_tiles, table, offsets, gtable, loss_scale, pr, tile,
-                                     const_cast<int32_t*>(counters));
+    for (uint32_t item = blockIdx.x; item < kLevelGroups * nt; item += gridDim.x) {
+        const uint32_t grp = item / nt;
+        encode_bwd_visit<SCATTER, TV>(p, recs, rays_o, rays_d, denc_tiles, table, offsets, gtable, loss_scale, pr, t0 + item % nt,
+                                      group_first_level(grp), group_first_level(grp + 1), const_cast<int32_t*>(counters));
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -727,6 +751,18 @@ static inline uint32_t part_grid(uint32_t Mcap, uint32_t nparts) {
     return nparts <= 1 ? Mcap / kTile : div_up(Mcap / kTile, nparts) + 1;
 }
 
+// blocks for one scatter / TV launch: the CTAs that are resident on the device at once (read once per process), so that the
+// group-major item order is also the order in which the items run; never more than the launch has items
+template <bool SCATTER, bool TV>
+static uint32_t encode_bwd_grid(uint32_t Mcap, uint32_t nparts) {
+    static int per_sm = 0;
+    if (!per_sm) {
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_s0_encode_bwd<SCATTER, TV>, kTile, 0);
+        if (per_sm <= 0) per_sm = 1;
+    }
+    return min((uint32_t)(per_sm * num_sms()), kLevelGroups * part_grid(Mcap, nparts));
+}
+
 extern "C" {
 
 /* test hook: 1 = one-thread-per-ray sequential marcher (the reference's structure), 0 = warp-per-ray (default) */
@@ -845,17 +881,9 @@ int n2m_s0_encode_bwd(const n2m_s0_params* p, const void* recs, const int32_t* c
     N2M_REQUIRE(p->num_levels == kLevels, "s0_encode_bwd", "fused path supports num_levels == 16");
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_encode_bwd", "Mcap must be a positive multiple of 128");
     N2M_REQUIRE(valid_parts(part, nparts), "s0_encode_bwd", "nparts must be 1, 2, 4 or 8 and part < nparts");
-    const float4* rc = static_cast<const float4*>(recs);
-    const uint8_t* dt = static_cast<const uint8_t*>(denc_tiles);
-    const TableEntry* tab = static_cast<const TableEntry*>(table);
-    float4* gt = static_cast<float4*>(gtable);
-    float* ls = const_cast<float*>(loss_scale);
-    if (nparts == 1)
-        k_s0_encode_bwd<true, false, false><<<Mcap / kTile, kTile, 0, as_stream(stream)>>>(*p, rc, counters, rays_o, rays_d, dt, tab, offsets,
-                                                                                           gt, ls, part, nparts);
-    else
-        k_s0_encode_bwd<true, false, true><<<part_grid(Mcap, nparts), kTile, 0, as_stream(stream)>>>(*p, rc, counters, rays_o, rays_d, dt, tab,
-                                                                                                     offsets, gt, ls, part, nparts);
+    k_s0_encode_bwd<true, false><<<encode_bwd_grid<true, false>(Mcap, nparts), kTile, 0, as_stream(stream)>>>(
+        *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, static_cast<const uint8_t*>(denc_tiles),
+        static_cast<const TableEntry*>(table), offsets, static_cast<float4*>(gtable), const_cast<float*>(loss_scale), part, nparts);
     return check_launch("s0_encode_bwd");
 }
 
@@ -866,10 +894,9 @@ int n2m_s0_tv(const n2m_s0_params* p, const void* recs, const int32_t* counters,
     N2M_REQUIRE(p && recs && counters && rays_o && rays_d && table && offsets && gtable && loss_scale, "s0_tv", "null pointer");
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_tv", "Mcap must be a positive multiple of 128");
     if (!(p->lambda_tv > 0)) return 0;
-    k_s0_encode_bwd<false, true, false><<<Mcap / kTile, kTile, 0, as_stream(stream)>>>(*p, static_cast<const float4*>(recs), counters, rays_o,
-                                                                                        rays_d, nullptr, static_cast<const TableEntry*>(table),
-                                                                                        offsets, static_cast<float4*>(gtable),
-                                                                                        const_cast<float*>(loss_scale), 0, 1);
+    k_s0_encode_bwd<false, true><<<encode_bwd_grid<false, true>(Mcap, 1), kTile, 0, as_stream(stream)>>>(
+        *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, nullptr, static_cast<const TableEntry*>(table), offsets,
+        static_cast<float4*>(gtable), const_cast<float*>(loss_scale), 0, 1);
     return check_launch("s0_tv");
 }
 

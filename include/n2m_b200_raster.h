@@ -12,7 +12,13 @@
  *       cross the camera plane (some w <= 0) are rasterised in homogeneous coordinates (the part in front of the near plane).
  *   n2m_interpolate_forward   dr.interpolate(attr, rast, tri)         (renderer.py:862-863): out [H*W,A] = u a0 + v a1 + (1-u-v) a2
  *   n2m_interpolate_backward  its gradient w.r.t. attr [V,A] (accumulated into the caller's zero-initialised buffer)
- *   n2m_compact_covered       xyzs[mask], dirs[mask] of renderer.py:865-880 without the boolean-mask host sync: covered pixel
+ *   n2m_interpolate_backward_rast  its gradient w.r.t. rast: grad_rast [H*W,4] = (du, dv, 0, 0) with du = sum_a g_a (a0_a - a2_a),
+ *                             dv = sum_a g_a (a1_a - a2_a) at covered pixels, zeros elsewhere (written, not accumulated)
+ *   n2m_rasterize_backward    dr.rasterize's gradient w.r.t. pos, as nvdiffrast defines it: only the (u, v) channels of grad_rast [H*W,4]
+ *       carry gradient; (u, v) = (a0, a1) / (a0 + a1 + a2) with the edge functions a_k = p'_{k+1} x p'_{k+2} of p'_k = (x_k - X w_k,
+ *       y_k - Y w_k) at the pixel's NDC centre (X, Y) -- the same expression for triangles that cross the camera plane.  d/d(x, y, w)
+ *       ACCUMULATED into the caller's grad_pos [V,4]; clip z gets nothing.
+ *   n2m_compact_covered      xyzs[mask], dirs[mask] of renderer.py:865-880 without the boolean-mask host sync: covered pixel
  *                             indices + their positions / view directions, count in *counter (device)
  *   n2m_antialias_*           dr.antialias(color, rast, pos, tri, pos_gradient_boost=b)   (renderer.py:886-887), csrc/antialias.cu:
  *       topology: edge -> opposing-vertex hash of the mesh (the library's "topology hash"), `keys` [slots] u64 and `opp` [2*slots] i32
@@ -25,6 +31,7 @@
 #define N2M_B200_RASTER_H
 
 #include "n2m_b200.h"
+#include "n2m_b200_fused.h"   /* n2m_s0_params (n2m_s1_offset_grad) */
 
 #ifdef __cplusplus
 extern "C" {
@@ -36,6 +43,10 @@ int n2m_interpolate_forward(const float* attr, uint32_t V, uint32_t A, const flo
                             float* out, n2m_stream_t stream);
 int n2m_interpolate_backward(const float* grad_out, const float* rast, const int32_t* tri, uint32_t num_pixels, uint32_t V, uint32_t A,
                              float* grad_attr, n2m_stream_t stream);
+int n2m_interpolate_backward_rast(const float* grad_out, const float* attr, const float* rast, const int32_t* tri, uint32_t num_pixels, uint32_t A,
+                                  float* grad_rast, n2m_stream_t stream);
+int n2m_rasterize_backward(const float* pos, uint32_t V, const int32_t* tri, const float* rast, const float* grad_rast, uint32_t H, uint32_t W,
+                           float* grad_pos, n2m_stream_t stream);
 int n2m_compact_covered(const float* rast, const float* xyz, const float* dirs, uint32_t num_pixels, uint32_t cap, int32_t* counter,
                         int32_t* pix, float* pts, float* pdirs, n2m_stream_t stream);
 
@@ -102,6 +113,23 @@ int n2m_s1_vert_check(const float* grad_vclip, uint32_t V, float* opt_state, n2m
 int n2m_s1_vert_step(const float* grad_vclip, const float* mvp, const void* topo_keys, uint32_t topo_slots, const float* base, float* offsets,
                      float* m, float* v, float* vertices, float* scratch, float* grad_out, uint32_t V, float lambda_lap, float lambda_offsets,
                      float lr_vert, float eps, const float* opt_state, float* vert_state, float* loss_out, n2m_stream_t stream);
+
+/* colour-field path of the vertex gradient (--enable_offset_nerf_grad: renderer.py:877-879 with xyzs[mask_flatten] not detached).
+ * n2m_s1_offset_grad (after n2m_s0_mlp_bwd, before n2m_s1_vert_check): for every super-sampled pixel with a point (inv[i] >= 0), the
+ * loss-scaled gradient w.r.t. its surface point = the colour-net input columns kColXyz..+2 of its denc_tiles row + the colour hash grid's
+ * input gradient (the reference's dy_dx over the fp16 colour features of `table`, zero outside [0,1]^3), through the Jacobian of
+ * contract() when p->contract; then dr.interpolate's backward: b_k dx ACCUMULATED into grad_vworld [V,3] (world space), and (du, dv)
+ * through n2m_rasterize_backward's expression ACCUMULATED into grad_vclip [V,4] (clip space, beside n2m_antialias_backward's gradient).
+ * rast [h,w,4], verts [V,3], vclip [V,4], tri, inv, pts: those of the step (n2m_rasterize, n2m_s1_points).  A non-finite gradient sets
+ * found_inf (opt_state[3]) and is not scattered.  p->num_levels must be 16.
+ * n2m_s1_vert_step_world: n2m_s1_vert_step with the image-loss part (grad_vclip . mvp[:, :3] + grad_vworld) / loss_scale. */
+int n2m_s1_offset_grad(const n2m_s0_params* p,const float* rast, const float* verts, const float* vclip, const int32_t* tri, const int32_t* inv,
+                       uint32_t h, uint32_t w, const float* pts, const void* denc_tiles, const void* table, const int32_t* offsets,
+                       float* grad_vclip, float* grad_vworld, float* opt_state, n2m_stream_t stream);
+int n2m_s1_vert_step_world(const float* grad_vclip, const float* grad_vworld, const float* mvp, const void* topo_keys, uint32_t topo_slots,
+                           const float* base, float* offsets, float* m, float* v, float* vertices, float* scratch, float* grad_out, uint32_t V,
+                           float lambda_lap, float lambda_offsets, float lr_vert, float eps, const float* opt_state, float* vert_state,
+                           float* loss_out, n2m_stream_t stream);
 
 #ifdef __cplusplus
 }

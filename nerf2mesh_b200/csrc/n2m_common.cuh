@@ -57,6 +57,23 @@ __device__ __forceinline__ void contract_linf(float p[3]) {
     }
 }
 
+// Backward of contract_linf at the UNcontracted point x: g <- J(x)^T g.  Outside the unit cube y = x s(m), m = max_k |x_k|,
+// s(m) = (2 - 1/m) / m, so J^T g = s g + (g . x) s'(m) dm/dx with s'(m) = 2 (1 - m) / m^3; dm/dx_k = sign(x_k) / t on the t components
+// that attain the maximum and 0 elsewhere -- torch's amax backward splits the gradient evenly between ties.
+__device__ __forceinline__ void contract_linf_backward(const float x[3], float g[3]) {
+    const float ax = fabsf(x[0]), ay = fabsf(x[1]), az = fabsf(x[2]);
+    const float m = fmaxf(ax, fmaxf(ay, az));
+    if (!(m > 1.f)) return;
+    const float r = 1.f / m;
+    const float s = (2.f - r) * r;
+    const float gx = g[0] * x[0] + g[1] * x[1] + g[2] * x[2];
+    const float t = (float)((ax == m) + (ay == m) + (az == m));
+    const float c = gx * 2.f * (1.f - m) * r * r * r / t;
+    const float a[3] = {ax, ay, az};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) g[k] = s * g[k] + (a[k] == m ? (x[k] < 0.f ? -c : c) : 0.f);
+}
+
 // 11-bit -> 31-bit spread for 3D Morton codes (bit i of v lands at bit 3i).  Identical to the
 // reference's multiply-and-mask form (raymarching.cu:56-63) for every v < 2048 (checked
 // exhaustively in tests/test_host_logic.py); the reference documents coords in [0,128).

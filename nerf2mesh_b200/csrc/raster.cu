@@ -15,6 +15,8 @@
 //   k_rast_resolve   : one thread per pixel: decode the winner, recompute its screen-space barycentrics with the SAME fp32 expressions,
 //                      make them perspective-correct with the clip-space w, write (u, v, z/w, id + 1) as one float4
 //   k_interp_fwd/bwd : attr = u a0 + v a1 + (1-u-v) a2 per pixel; backward scatters to the three vertices with red.global.add
+//   k_interp_bwd_rast, k_rast_bwd : the gradients of interpolate w.r.t. rast's (u, v) and of rasterize w.r.t. pos through (u, v), as
+//                      nvdiffrast defines them (arithmetic in raster_grad.cuh, shared with the stage-1 step's k_s1_offset_grad)
 // Near / far clipping: triangles in front of the camera plane (all w > 0) are tested per pixel against -1 <= z/w <= 1.  Triangles that
 // CROSS the camera plane (some w <= 0: ground or shell triangles around a camera inside the scene) are rasterised in 2-D homogeneous
 // coordinates (Olano & Greer 1997): for pixel NDC (X, Y) the solution of sum_i b'_i (x_i, y_i, w_i) = (X, Y, 1) is non-negative exactly
@@ -22,6 +24,7 @@
 // -- the result of clipping against the near plane without building clipped polygons; only the bounding box comes from the clipped
 // outline.  Not reproduced (oracle/raster_oracle.py): the exact OpenGL top-left fill rule for pixel centres exactly on an edge.
 #include "n2m_common.cuh"
+#include "raster_grad.cuh"
 #include "../../include/n2m_b200_raster.h"
 
 namespace n2m {
@@ -240,6 +243,46 @@ k_interp_bwd(const float* __restrict__ grad_out, const float4* __restrict__ rast
     }
 }
 
+// dr.rasterize backward: one thread per pixel, d loss / d (u, v) of the covered pixels -> grad_pos [V,4] (raster_grad.cuh)
+__global__ void __launch_bounds__(256)
+k_rast_bwd(const float4* __restrict__ pos, const int32_t* __restrict__ tri, const float4* __restrict__ rast, const float4* __restrict__ grad_rast,
+           uint32_t H, uint32_t W, float* __restrict__ grad_pos) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= H * W) return;
+    const float4 r = rast[i];
+    if (!(r.w > 0.f)) return;
+    const float4 g = grad_rast[i];
+    if (g.x == 0.f && g.y == 0.f) return;
+    const uint32_t f = (uint32_t)r.w - 1u;
+    const int vi[3] = {tri[3 * f], tri[3 * f + 1], tri[3 * f + 2]};
+    const float4 p[3] = {__ldg(pos + vi[0]), __ldg(pos + vi[1]), __ldg(pos + vi[2])};
+    const float2 ndc = pixel_ndc(i % W, i / W, H, W);
+    rasterize_uv_backward(p, vi, ndc.x, ndc.y, g.x, g.y, grad_pos);
+}
+
+// dr.interpolate backward w.r.t. rast: grad_rast [n,4] = (du, dv, 0, 0) at covered pixels, zeros elsewhere (raster_grad.cuh)
+template <int A>
+__global__ void __launch_bounds__(256)
+k_interp_bwd_rast(const float* __restrict__ grad_out, const float* __restrict__ attr, const float4* __restrict__ rast, const int32_t* __restrict__ tri,
+                  uint32_t n, float4* __restrict__ grad_rast) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 r = rast[i];
+    float2 d = make_float2(0.f, 0.f);
+    if (r.w > 0.f) {
+        const uint32_t f = (uint32_t)r.w - 1u;
+        const int i0 = tri[3 * f], i1 = tri[3 * f + 1], i2 = tri[3 * f + 2];
+        float g[A], a0[A], a1[A], a2[A];
+#pragma unroll
+        for (int a = 0; a < A; ++a) {
+            g[a] = grad_out[(size_t)i * A + a];
+            a0[a] = __ldg(attr + (size_t)i0 * A + a); a1[a] = __ldg(attr + (size_t)i1 * A + a); a2[a] = __ldg(attr + (size_t)i2 * A + a);
+        }
+        d = interpolate_uv_backward<A>(g, a0, a1, a2);
+    }
+    grad_rast[i] = make_float4(d.x, d.y, 0.f, 0.f);
+}
+
 // covered-pixel compaction for the texture-MLP step (renderer.py:865-880: xyzs[mask_flatten], dirs[mask_flatten]): one thread per
 // pixel, warp-aggregated atomic counter; writes the pixel index, its interpolated position and its (unnormalised) view direction
 __global__ void __launch_bounds__(256)
@@ -322,6 +365,35 @@ int n2m_interpolate_backward(const float* grad_out, const float* rast, const int
         default: return fail("interpolate_backward", "attribute count must be 1..4");
     }
     return check_launch("interpolate_backward");
+}
+
+int n2m_rasterize_backward(const float* pos, uint32_t V, const int32_t* tri, const float* rast, const float* grad_rast, uint32_t H, uint32_t W,
+                           float* grad_pos, n2m_stream_t stream) {
+    N2M_REQUIRE(pos && tri && rast && grad_rast && grad_pos, "rasterize_backward", "null pointer");
+    N2M_REQUIRE((uint64_t)H * W < (1ull << 31), "rasterize_backward", "bad resolution");
+    (void)V;
+    if (H == 0 || W == 0) return 0;
+    k_rast_bwd<<<div_up(H * W, 256u), 256, 0, as_stream(stream)>>>(reinterpret_cast<const float4*>(pos), tri, reinterpret_cast<const float4*>(rast),
+                                                                   reinterpret_cast<const float4*>(grad_rast), H, W, grad_pos);
+    return check_launch("rasterize_backward");
+}
+
+int n2m_interpolate_backward_rast(const float* grad_out, const float* attr, const float* rast, const int32_t* tri, uint32_t num_pixels, uint32_t A,
+                                  float* grad_rast, n2m_stream_t stream) {
+    N2M_REQUIRE(grad_out && attr && rast && tri && grad_rast, "interpolate_backward_rast", "null pointer");
+    if (num_pixels == 0) return 0;
+    const float4* r = reinterpret_cast<const float4*>(rast);
+    float4* gr = reinterpret_cast<float4*>(grad_rast);
+    cudaStream_t st = as_stream(stream);
+    const uint32_t g = div_up(num_pixels, 256u);
+    switch (A) {
+        case 1: k_interp_bwd_rast<1><<<g, 256, 0, st>>>(grad_out, attr, r, tri, num_pixels, gr); break;
+        case 2: k_interp_bwd_rast<2><<<g, 256, 0, st>>>(grad_out, attr, r, tri, num_pixels, gr); break;
+        case 3: k_interp_bwd_rast<3><<<g, 256, 0, st>>>(grad_out, attr, r, tri, num_pixels, gr); break;
+        case 4: k_interp_bwd_rast<4><<<g, 256, 0, st>>>(grad_out, attr, r, tri, num_pixels, gr); break;
+        default: return fail("interpolate_backward_rast", "attribute count must be 1..4");
+    }
+    return check_launch("interpolate_backward_rast");
 }
 
 int n2m_compact_covered(const float* rast, const float* xyz, const float* dirs, uint32_t num_pixels, uint32_t cap, int32_t* counter,

@@ -195,6 +195,11 @@ encode_fwd_features(const n2m_s0_params& p, const float4* __restrict__ recs, con
     return own;
 }
 
+// one fp16 gradient column of a tile-image row (`row` = the row's first byte in chunk 0)
+__device__ __forceinline__ float denc_col(const uint8_t* row, uint32_t col) {
+    return __half2float(__ldg(reinterpret_cast<const __half*>(row + (col >> 3) * kChunkBytes + (col & 7) * 2)));
+}
+
 // row r of a tile image at `img` (global or shared): 8 chunks of 16 bytes, each chunk 2 KiB apart
 __device__ __forceinline__ void store_tile_row(uint8_t* img, uint32_t r, const float (&feat)[kTileCols]) {
     uint8_t* dst = img + r * 16;

@@ -307,11 +307,6 @@ __device__ __forceinline__ void red_add_v4(float4* dst, float a, float b, float 
                  :: "l"(dst), "f"(a), "f"(b), "f"(c), "f"(0.f), "l"(pol) : "memory");
 }
 
-// one fp16 gradient column of a tile-image row (`row` = the row's first byte in chunk 0)
-__device__ __forceinline__ float denc_col(const uint8_t* row, uint32_t col) {
-    return __half2float(__ldg(reinterpret_cast<const __half*>(row + (col >> 3) * kChunkBytes + (col & 7) * 2)));
-}
-
 template <bool SCATTER, bool TV>
 __device__ __forceinline__ void
 encode_bwd_visit(const n2m_s0_params& p, const float4* __restrict__ recs,

@@ -19,9 +19,15 @@
 //   n2m_s1_loss_aa                    clamp, alphas * rgbs, ssaa average, background mix, loss; gradient w.r.t. the antialiased image
 //   n2m_antialias_backward            -> gradient w.r.t. the (r, g, b, mask) image and w.r.t. the clip-space vertices (vertices_offsets)
 //   n2m_s1_dout                       gather of the colour gradient back to the compacted points
+// With --enable_offset_nerf_grad (xyzs not detached, renderer.py:877-879) the backward adds
+//   n2m_s1_offset_grad                after the MLP backward: every point's colour-net + colour-grid input gradient (through contract()),
+//                                     back through dr.interpolate and dr.rasterize's (u, v) to the vertices (grad_vworld, grad_vclip)
+// and the vertex step becomes n2m_s1_vert_step_world.
 // With mesh refinement on (opt.refine), n2m_s1_loss_err / n2m_s1_loss_aa_err replace the two loss launches: the same kernels, which also
 // accumulate each pixel's loss and a hit into the face it sees (update_triangles_errors, renderer.py:893-903,923-943; utils.py:720-721).
 #include "n2m_common.cuh"
+#include "raster_grad.cuh"
+#include "s0_geom.cuh"
 #include "../../include/n2m_b200_raster.h"
 
 namespace n2m {
@@ -256,6 +262,93 @@ k_s1_loss_aa(const float4* __restrict__ aa, const float* __restrict__ gt, uint32
     }
 }
 
+// ---- colour-field path of the vertex gradient (--enable_offset_nerf_grad: renderer.py:877-879 with xyzs[mask_flatten] not detached) ----
+// One thread per super-sampled pixel with a point (inv[i] >= 0).  The loss-scaled gradient w.r.t. the point the colour field saw is
+//   the direct term: tile columns kColXyz..+2 of its denc row (x is an input of color_net.0; dS1 is zero in stage 1), plus
+//   the hash-grid term: per level, d(colour feature)/du of the trilinear interpolation (the reference's dy_dx, gridencoder.cu:198-240:
+//   per dimension the weights of the other two dimensions times (right - left corner) times the level scale) dotted with the feature's
+//   denc columns, times inv_2gb for u = (x + bound) / (2 bound); zero outside [0,1]^3, where the encoder outputs zeros;
+// CONTRACT: then through the Jacobian of contract() at the uncontracted point (recomputed from rast and the vertices as k_s1_points
+// does).  The scatter is dr.interpolate's backward: b_k dx into grad_vworld [V,3], and (du, dv) through dr.rasterize's backward into
+// grad_vclip [V,4] beside the antialias gradient (raster_grad.cuh).  A non-finite gradient (fp16 overflow of the x columns) sets found_inf
+// (st[3]) and is not scattered.
+template <bool CONTRACT>
+__global__ void __launch_bounds__(256)
+k_s1_offset_grad(const n2m_s0_params p, const float4* __restrict__ rast, const float* __restrict__ verts, const float4* __restrict__ vclip,
+                 const int32_t* __restrict__ tri, const int32_t* __restrict__ inv, uint32_t h, uint32_t w, const float* __restrict__ pts,
+                 const uint8_t* __restrict__ denc_tiles, const TableEntry* __restrict__ table, const int32_t* __restrict__ offsets,
+                 float* __restrict__ grad_vclip, float* __restrict__ grad_vworld, float* __restrict__ st) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= h * w) return;
+    const int32_t k = inv[i];
+    if (k < 0) return;
+    const uint8_t* img = denc_tiles + (size_t)(k / kTile) * kTileBytes + (k % kTile) * 16;
+    float g[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) g[a] = denc_col(img, kColXyz + a);
+    const float x = pts[3 * (size_t)k], y = pts[3 * (size_t)k + 1], z = pts[3 * (size_t)k + 2];
+    const float u = __fmul_rn(__fadd_rn(x, p.grid_bound), p.inv_2gb);       // encode_fwd_features (POINTS)
+    const float v = __fmul_rn(__fadd_rn(y, p.grid_bound), p.inv_2gb);
+    const float ww = __fmul_rn(__fadd_rn(z, p.grid_bound), p.inv_2gb);
+    if (!((u < 0 || u > 1) || (v < 0 || v > 1) || (ww < 0 || ww > 1))) {
+        float gu[3] = {0.f, 0.f, 0.f};
+#pragma unroll 1
+        for (uint32_t l = 0; l < kLevels; ++l) {
+            const float g0 = denc_col(img, kColColor + 2 * l), g1 = denc_col(img, kColColor + 2 * l + 1);
+            const LevelGeom lg = level_geom(offsets, l, p.S, p.base_res);
+            Corners c; uint32_t base[3]; bool hashed;
+            corners_of(lg, u, v, ww, c, base, hashed, nullptr);
+            const float fr[3] = {(u * lg.scale + 0.5f) - (float)base[0], (v * lg.scale + 0.5f) - (float)base[1], (ww * lg.scale + 0.5f) - (float)base[2]};
+            const TableEntry* tab = table + lg.row0;
+            float f[8];
+#pragma unroll
+            for (int q = 0; q < 8; ++q) {
+                const uint2 raw = __ldg(reinterpret_cast<const uint2*>(tab + c.row[q]));
+                const float2 cc = __half22float2(*reinterpret_cast<const __half2*>(&raw.y));
+                f[q] = g0 * cc.x + g1 * cc.y;                  // the feature gradient dotted with the corner's two features
+            }
+#pragma unroll
+            for (int d = 0; d < 3; ++d) {
+                const int d1 = (d + 1) % 3, d2 = (d + 2) % 3;
+                float s = 0.f;
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    const float w1 = ((q >> d1) & 1) ? fr[d1] : 1.f - fr[d1], w2 = ((q >> d2) & 1) ? fr[d2] : 1.f - fr[d2];
+                    s += ((q >> d) & 1) ? w1 * w2 * f[q] : -(w1 * w2 * f[q]);
+                }
+                gu[d] += lg.scale * s;
+            }
+        }
+#pragma unroll
+        for (int a = 0; a < 3; ++a) g[a] += gu[a] * p.inv_2gb;
+    }
+    const float4 r = rast[i];
+    const uint32_t f = (uint32_t)r.w - 1u;
+    const int vi[3] = {tri[3 * f], tri[3 * f + 1], tri[3 * f + 2]};
+    float vx[3][3];
+#pragma unroll
+    for (int q = 0; q < 3; ++q)
+#pragma unroll
+        for (int a = 0; a < 3; ++a) vx[q][a] = __ldg(verts + 3 * (size_t)vi[q] + a);
+    if constexpr (CONTRACT) {
+        float xu[3];
+        const float bw = 1.f - r.x - r.y;
+#pragma unroll
+        for (int a = 0; a < 3; ++a) xu[a] = r.x * vx[0][a] + r.y * vx[1][a] + bw * vx[2][a];
+        contract_linf_backward(xu, g);
+    }
+    if (!(isfinite(g[0]) && isfinite(g[1]) && isfinite(g[2]))) { st[3] = 1.f; return; }
+    const float b[3] = {r.x, r.y, 1.f - r.x - r.y};
+#pragma unroll
+    for (int q = 0; q < 3; ++q)
+#pragma unroll
+        for (int a = 0; a < 3; ++a) atomicAdd(grad_vworld + 3 * (size_t)vi[q] + a, b[q] * g[a]);
+    const float2 duv = interpolate_uv_backward<3>(g, vx[0], vx[1], vx[2]);
+    const float4 pc[3] = {__ldg(vclip + vi[0]), __ldg(vclip + vi[1]), __ldg(vclip + vi[2])};
+    const float2 ndc = pixel_ndc(i % w, i / w, h, w);
+    rasterize_uv_backward(pc, vi, ndc.x, ndc.y, duv.x, duv.y, grad_vclip);
+}
+
 // ---- vertex-offset optimizer (NeRFRenderer.vertices_offsets: renderer.py:160,180 -- Adam group with lr_vert; regularisers
 // utils.py:750-779: lambda_lap * laplacian_smooth_loss (uniform Laplacian, utils.py:176-221) + lambda_offsets * mean(sum(offsets^2))) ----
 // y += L x for the uniform Laplacian L = D - A, one thread per slot of the edge hash of csrc/antialias.cu (one slot = one undirected edge)
@@ -299,11 +392,15 @@ k_s1_vert_check(const float* __restrict__ g, uint32_t n, float* __restrict__ st)
 }
 
 // grad = (grad_vclip . mvp[:, :3]) / loss_scale + (lambda_lap / V) * (L w) + (2 lambda_offsets / V) * offsets; Adam(eps) on the offsets with
-// its own step count vst[0]; vertices = base + offsets.  Skipped as a whole when found_inf is set (st[3]).
+// its own step count vst[0]; vertices = base + offsets.  Skipped as a whole when found_inf is set (st[3]).  WORLD: the image-loss part is
+// (grad_vclip . mvp[:, :3] + grad_vworld) / loss_scale (the colour-field path, k_s1_offset_grad); grad_vworld is the last parameter, so
+// the WORLD = false instantiation keeps the parameter offsets, and the code, of the kernel without it.
+template <bool WORLD>
 __global__ void __launch_bounds__(256)
 k_s1_vert_adam(const float4* __restrict__ grad_vclip, const float* __restrict__ mvp, const float* __restrict__ lap_grad, const float* __restrict__ base,
                float* __restrict__ offsets, float* __restrict__ m, float* __restrict__ v, float* __restrict__ vertices, float* __restrict__ grad_out,
-               uint32_t V, float lambda_lap, float lambda_offsets, float lr, float eps, const float* __restrict__ st, const float* __restrict__ vst) {
+               uint32_t V, float lambda_lap, float lambda_offsets, float lr, float eps, const float* __restrict__ st, const float* __restrict__ vst,
+               const float* __restrict__ grad_vworld) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= V) return;
     if (lr < 0.f) lr = vst[1];                                          // learning rate kept on the device (graph-replayed steps)
@@ -315,7 +412,9 @@ k_s1_vert_adam(const float4* __restrict__ grad_vclip, const float* __restrict__ 
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
         const size_t j = 3 * (size_t)i + c;
-        const float gi = (gc.x * mvp[c] + gc.y * mvp[4 + c] + gc.z * mvp[8 + c] + gc.w * mvp[12 + c]) * inv_scale;
+        float gi;
+        if constexpr (WORLD) gi = (gc.x * mvp[c] + gc.y * mvp[4 + c] + gc.z * mvp[8 + c] + gc.w * mvp[12 + c] + grad_vworld[j]) * inv_scale;
+        else gi = (gc.x * mvp[c] + gc.y * mvp[4 + c] + gc.z * mvp[8 + c] + gc.w * mvp[12 + c]) * inv_scale;
         const float off = offsets[j];
         const float g = gi + (lambda_lap > 0.f ? lambda_lap / (float)V * lap_grad[j] : 0.f) + 2.f * lambda_offsets / (float)V * off;
         if (grad_out) grad_out[j] = g;
@@ -438,9 +537,25 @@ int n2m_s1_vert_check(const float* grad_vclip, uint32_t V, float* opt_state, n2m
     return check_launch("s1_vert_check");
 }
 
-int n2m_s1_vert_step(const float* grad_vclip, const float* mvp, const void* topo_keys, uint32_t topo_slots, const float* base, float* offsets,
-                     float* m, float* v, float* vertices, float* scratch, float* grad_out, uint32_t V, float lambda_lap, float lambda_offsets,
-                     float lr_vert, float eps, const float* opt_state, float* vert_state, float* loss_out, n2m_stream_t stream) {
+int n2m_s1_offset_grad(const n2m_s0_params* p, const float* rast, const float* verts, const float* vclip, const int32_t* tri, const int32_t* inv,
+                       uint32_t h, uint32_t w, const float* pts, const void* denc_tiles, const void* table, const int32_t* offsets,
+                       float* grad_vclip, float* grad_vworld, float* opt_state, n2m_stream_t stream) {
+    N2M_REQUIRE(p && rast && verts && vclip && tri && inv && pts && denc_tiles && table && offsets && grad_vclip && grad_vworld && opt_state,
+                "s1_offset_grad", "null pointer");
+    N2M_REQUIRE(p->num_levels == kLevels, "s1_offset_grad", "the colour grid must have 16 levels");
+    N2M_REQUIRE((uint64_t)h * w < (1ull << 31), "s1_offset_grad", "bad resolution");
+    if (h == 0 || w == 0) return 0;
+    auto kernel = p->contract ? k_s1_offset_grad<true> : k_s1_offset_grad<false>;
+    kernel<<<div_up(h * w, 256u), 256, 0, as_stream(stream)>>>(*p, reinterpret_cast<const float4*>(rast), verts, reinterpret_cast<const float4*>(vclip),
+                                                                tri, inv, h, w, pts, static_cast<const uint8_t*>(denc_tiles),
+                                                                static_cast<const TableEntry*>(table), offsets, grad_vclip, grad_vworld, opt_state);
+    return check_launch("s1_offset_grad");
+}
+
+static int s1_vert_step(const float* grad_vclip, const float* grad_vworld, const float* mvp, const void* topo_keys, uint32_t topo_slots,
+                        const float* base, float* offsets, float* m, float* v, float* vertices, float* scratch, float* grad_out, uint32_t V,
+                        float lambda_lap, float lambda_offsets, float lr_vert, float eps, const float* opt_state, float* vert_state, float* loss_out,
+                        n2m_stream_t stream) {
     N2M_REQUIRE(grad_vclip && mvp && base && offsets && m && v && vertices && scratch && opt_state && vert_state, "s1_vert_step", "null pointer");
     N2M_REQUIRE(lambda_lap <= 0.f || (topo_keys && topo_slots > 0), "s1_vert_step", "the Laplacian term needs the mesh's edge hash");
     if (V == 0) return 0;
@@ -458,11 +573,28 @@ int n2m_s1_vert_step(const float* grad_vclip, const float* mvp, const void* topo
         k_s1_laplacian<<<div_up(topo_slots, 256u), 256, 0, st>>>(keys, topo_slots, u, lg);
         if (int err = check_launch("s1_vert_step(L w)")) return err;
     }
-    k_s1_vert_adam<<<div_up(V, 256u), 256, 0, st>>>(reinterpret_cast<const float4*>(grad_vclip), mvp, lg, base, offsets, m, v, vertices, grad_out, V,
-                                                   lambda_lap, lambda_offsets, lr_vert, eps, opt_state, vert_state);
+    auto adam = grad_vworld ? k_s1_vert_adam<true> : k_s1_vert_adam<false>;
+    adam<<<div_up(V, 256u), 256, 0, st>>>(reinterpret_cast<const float4*>(grad_vclip), mvp, lg, base, offsets, m, v, vertices, grad_out, V,
+                                          lambda_lap, lambda_offsets, lr_vert, eps, opt_state, vert_state, grad_vworld);
     if (int err = check_launch("s1_vert_step(adam)")) return err;
     k_s1_vert_tick<<<1, 32, 0, st>>>(opt_state, vert_state);
     return check_launch("s1_vert_step(tick)");
+}
+
+int n2m_s1_vert_step(const float* grad_vclip, const float* mvp, const void* topo_keys, uint32_t topo_slots, const float* base, float* offsets,
+                     float* m, float* v, float* vertices, float* scratch, float* grad_out, uint32_t V, float lambda_lap, float lambda_offsets,
+                     float lr_vert, float eps, const float* opt_state, float* vert_state, float* loss_out, n2m_stream_t stream) {
+    return s1_vert_step(grad_vclip, nullptr, mvp, topo_keys, topo_slots, base, offsets, m, v, vertices, scratch, grad_out, V, lambda_lap,
+                        lambda_offsets, lr_vert, eps, opt_state, vert_state, loss_out, stream);
+}
+
+int n2m_s1_vert_step_world(const float* grad_vclip, const float* grad_vworld, const float* mvp, const void* topo_keys, uint32_t topo_slots,
+                           const float* base, float* offsets, float* m, float* v, float* vertices, float* scratch, float* grad_out, uint32_t V,
+                           float lambda_lap, float lambda_offsets, float lr_vert, float eps, const float* opt_state, float* vert_state,
+                           float* loss_out, n2m_stream_t stream) {
+    N2M_REQUIRE(grad_vworld, "s1_vert_step_world", "null pointer");
+    return s1_vert_step(grad_vclip, grad_vworld, mvp, topo_keys, topo_slots, base, offsets, m, v, vertices, scratch, grad_out, V, lambda_lap,
+                        lambda_offsets, lr_vert, eps, opt_state, vert_state, loss_out, stream);
 }
 
 }  // extern "C"

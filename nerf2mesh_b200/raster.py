@@ -2,14 +2,17 @@
 
     glctx = RasterizeCudaContext()
     rast, rast_db = rasterize(glctx, pos, tri, (h, w))          # pos [1,V,4] clip space, tri [F,3] int32 -> rast [1,h,w,4]
-    out, out_db   = interpolate(attr, rast, tri)                 # attr [1,V,A] -> [1,h,w,A], differentiable w.r.t. attr
+    out, out_db   = interpolate(attr, rast, tri)                 # attr [1,V,A] -> [1,h,w,A], differentiable w.r.t. attr and rast
     img           = antialias(color, rast, pos, tri, pos_gradient_boost=1.0)   # color [1,h,w,C]; differentiable w.r.t. color and pos
 
 over the sm_90a kernels of csrc/raster.cu and csrc/antialias.cu (C ABI: include/n2m_b200_raster.h).
 `rast[..., :] = (u, v, z/w, triangle_id + 1)`.
-Not provided: image-space derivative outputs (`rast_db`, `out_db` are None: the reference ignores them, renderer.py:860-863) and
-gradients of rasterize w.r.t. vertex positions through (u, v) (the reference detaches `xyzs` unless enable_offset_nerf_grad,
-renderer.py:877; the silhouette gradient of `antialias` is the path it relies on).
+`rasterize` and `interpolate` are differentiable as nvdiffrast's are: the gradient of interpolate w.r.t. rast's (u, v) goes on
+through rasterize's (u, v) gradient to pos (clip x, y, w; z/w and the triangle id carry none).  rast stays a plain tensor: interpolate
+applies both steps of that chain rule in its backward, for a rast that rasterize made from a pos that requires grad.  That is the path of the reference's
+--enable_offset_nerf_grad (renderer.py:877-879: `xyzs` not detached); in its default composition the only differentiable use of rast is
+interpolate(ones) for the mask, whose (u, v) gradient is exactly zero.
+Not provided: image-space derivative outputs (`rast_db`, `out_db` are None: the reference ignores them, renderer.py:860-863).
 No CPU fallback: tensors must live on a CUDA device.
 """
 import torch
@@ -21,6 +24,8 @@ _lib.register({
     "n2m_rasterize": [P, U, P, U, U, U, P, P, P, P],
     "n2m_interpolate_forward": [P, U, U, P, P, U, P, P],
     "n2m_interpolate_backward": [P, P, P, U, U, U, P, P],
+    "n2m_interpolate_backward_rast": [P, P, P, P, U, U, P, P],
+    "n2m_rasterize_backward": [P, U, P, P, P, U, U, P, P],
     "n2m_compact_covered": [P, P, P, U, U, P, P, P, P, P],
     "n2m_antialias_topology": [P, U, P, P, U, P],
     "n2m_antialias_forward": [P, P, P, P, P, P, U, U, U, U, P, P],
@@ -50,7 +55,9 @@ RasterizeGLContext = RasterizeCudaContext        # the reference picks either (r
 
 
 def rasterize(glctx, pos, tri, resolution, ranges=None, grad_db=True):
-    """dr.rasterize: pos [1,V,4] float32 clip space (or [V,4]), tri [F,3] int32, resolution (h, w) -> (rast [1,h,w,4], None)."""
+    """dr.rasterize: pos [1,V,4] float32 clip space (or [V,4]), tri [F,3] int32, resolution (h, w) -> (rast [1,h,w,4], None).
+    Differentiable w.r.t. pos through the (u, v) channels of rast, as nvdiffrast is, with the gradient applied where the reference
+    differentiates rast: `interpolate` (see _Interpolate).  rast itself is a plain tensor that can be read as data."""
     if ranges is not None:
         raise NotImplementedError("range mode is not used by the reference")
     if not pos.is_cuda:
@@ -59,33 +66,49 @@ def rasterize(glctx, pos, tri, resolution, ranges=None, grad_db=True):
         if pos.shape[0] != 1:
             raise NotImplementedError("instanced mode with minibatch > 1 is not used by the reference")
         pos = pos[0]
-    pos = pos.detach().float().contiguous()
+    pos_g = pos.float().contiguous()
+    pos = pos_g.detach()
     tri = tri.int().contiguous()
     h, w = int(resolution[0]), int(resolution[1])
     vis, queue = glctx.scratch(h * w, tri.shape[0])
     rast = torch.empty(1, h, w, 4, device=pos.device, dtype=torch.float32)
     call("n2m_rasterize", ptr(pos), pos.shape[0], ptr(tri), tri.shape[0], h, w, ptr(vis), ptr(queue), ptr(rast), stream())
+    if pos_g.requires_grad and torch.is_grad_enabled():
+        rast._n2m_raster_src = (pos_g, tri)          # the (u, v) of rast are a function of pos: interpolate differentiates through them
     return rast, None
 
 
 class _Interpolate(torch.autograd.Function):
+    """out = interpolate(attr, rast); pos (optional) is the clip-space input rast was rasterized from: the gradient w.r.t. rast's (u, v)
+    (n2m_interpolate_backward_rast) goes on through dr.rasterize's backward (n2m_rasterize_backward) to pos -- the chain rule through rast
+    evaluated inside one node, so that rast stays a plain tensor"""
+
     @staticmethod
-    def forward(ctx, attr, rast, tri):
+    def forward(ctx, attr, rast, tri, pos, raster_tri):
         V, A = attr.shape
         n = rast.shape[0] * rast.shape[1] * rast.shape[2]
         out = torch.empty(*rast.shape[:3], A, device=attr.device, dtype=torch.float32)
         call("n2m_interpolate_forward", ptr(attr), V, A, ptr(rast), ptr(tri), n, ptr(out), stream())
-        ctx.save_for_backward(rast, tri)
+        ctx.save_for_backward(attr, rast, tri, pos, raster_tri)
         ctx.dims = (V, A, n)
         return out
 
     @staticmethod
     def backward(ctx, grad_out):
-        rast, tri = ctx.saved_tensors
+        attr, rast, tri, pos, raster_tri = ctx.saved_tensors
         V, A, n = ctx.dims
-        g = torch.zeros(V, A, device=grad_out.device, dtype=torch.float32)
-        call("n2m_interpolate_backward", ptr(grad_out.float().contiguous()), ptr(rast), ptr(tri), n, V, A, ptr(g), stream())
-        return g, None, None
+        grad_out = grad_out.float().contiguous()
+        g = gp = None
+        if ctx.needs_input_grad[0]:
+            g = torch.zeros(V, A, device=grad_out.device, dtype=torch.float32)
+            call("n2m_interpolate_backward", ptr(grad_out), ptr(rast), ptr(tri), n, V, A, ptr(g), stream())
+        if pos is not None and ctx.needs_input_grad[3]:
+            gr = torch.empty_like(rast)
+            call("n2m_interpolate_backward_rast", ptr(grad_out), ptr(attr), ptr(rast), ptr(tri), n, A, ptr(gr), stream())
+            gp = torch.zeros_like(pos)
+            call("n2m_rasterize_backward", ptr(pos), pos.shape[0], ptr(raster_tri), ptr(rast), ptr(gr), rast.shape[1], rast.shape[2], ptr(gp),
+                 stream())
+        return g, None, None, gp, None
 
 
 def interpolate(attr, rast, tri, rast_db=None, diff_attrs=None):
@@ -95,7 +118,9 @@ def interpolate(attr, rast, tri, rast_db=None, diff_attrs=None):
     a = attr[0] if attr.dim() == 3 else attr
     if a.shape[-1] < 1 or a.shape[-1] > 4:
         raise RuntimeError("interpolate: 1..4 attributes per vertex are supported")
-    out = _Interpolate.apply(a.float().contiguous(), rast.contiguous(), tri.int().contiguous())
+    src = getattr(rast, "_n2m_raster_src", None)
+    pos, raster_tri = src if src is not None else (None, None)
+    out = _Interpolate.apply(a.float().contiguous(), rast.contiguous(), tri.int().contiguous(), pos, raster_tri)
     return out, None
 
 

@@ -11,6 +11,10 @@ the model state (hash tables, MLP weights, optimizer moments, GradScaler state) 
 image-loss gradient w.r.t. the vertices in `vertex_gradient()` -- the quantity the reference's vertex optimizer consumes.
 `lr_vert > 0` also trains the vertex offsets as the reference's default stage 1 does (`vertices_offsets`, renderer.py:160,180: an Adam
 group with lr_vert; regularisers lambda_lap * laplacian_smooth_loss (uniform) + lambda_offsets * mean(sum(offsets^2)), utils.py:750-779).
+`offset_nerf_grad=True` (needs lr_vert > 0) is the reference's --enable_offset_nerf_grad (renderer.py:877-879; main.py:62, on whenever
+--sdf is set, main.py:149): the surface points are not detached, so the image loss also reaches the vertices through the colour field --
+the colour-net and colour-grid input gradient of every covered super-sample, through contract() in unbounded scenes, then
+dr.interpolate and dr.rasterize's (u, v) (n2m_s1_offset_grad, after the MLP backward).  `vertex_gradient()` is then the sum of both paths.
 `refine=True` adds the error-guided mesh refinement of the reference's stage 1 (opt.refine, main.py:129-136): every step also adds each
 low-res pixel's loss and a hit to the face that pixel sees (update_triangles_errors, renderer.py:893-903,923-943, fused into the loss
 kernels) in `face_errors` / `face_counts`; `refine_mask()` turns them into the decimate / refine face mask of refine_and_decimate
@@ -45,6 +49,8 @@ _lib.register({
     "n2m_s1_dout": [P, P, U, P, P],
     "n2m_s1_vert_check": [P, U, P, P],
     "n2m_s1_vert_step": [P, P, P, U, P, P, P, P, P, P, P, U, F, F, F, F, P, P, P, P],
+    "n2m_s1_offset_grad": [P, P, P, P, P, P, U, U, P, P, P, P, P, P, P, P],
+    "n2m_s1_vert_step_world": [P, P, P, P, U, P, P, P, P, P, P, P, U, F, F, F, F, P, P, P, P],
 })
 
 
@@ -52,7 +58,7 @@ class Stage1Trainer:
     v_cumsum = f_cumsum = ()            # per-cascade vertex / face offsets, set by _set_cascades
 
     def __init__(self, t0, vertices, triangles, h0, w0, ssaa=2, max_points=None, lambda_mask=0.1, antialias=False, pos_gradient_boost=1.0,
-                 lr_vert=0.0, lambda_lap=0.001, lambda_offsets=0.1, refine=False):
+                 lr_vert=0.0, lambda_lap=0.001, lambda_offsets=0.1, refine=False, offset_nerf_grad=False):
         assert ssaa in (1, 2), "the ssaa average equals the reference's bilinear down-scale only at factors 1 and 2"
         self.t0 = t0
         dev = t0.device
@@ -89,6 +95,10 @@ class Stage1Trainer:
             if not self.antialias:
                 raise ValueError("the image loss reaches the vertices through dr.antialias only: lr_vert > 0 needs antialias=True")
             self.vert_state = torch.zeros(4, device=dev)                  # [0] Adam step count of this group, [1] current lr_vert
+        # --enable_offset_nerf_grad (main.py:62; on with --sdf, main.py:149): the image loss also reaches the vertices through the colour field
+        self.offset_nerf_grad = bool(offset_nerf_grad)
+        if self.offset_nerf_grad and not self.lr_vert > 0:
+            raise ValueError("offset_nerf_grad trains the vertex offsets: it needs lr_vert > 0 (and with it antialias=True)")
         self.refine = bool(refine)
         self._mesh_buffers()
         # the specular regulariser and TV are stage-0 losses (utils.py:726,735-738)
@@ -133,6 +143,8 @@ class Stage1Trainer:
             self.m_vert = torch.zeros(V, 3, device=dev); self.v_vert = torch.zeros(V, 3, device=dev)
             self.vert_scratch = torch.zeros(6 * V, device=dev)
             self.grad_offsets = torch.zeros(V, 3, device=dev)             # total gradient of the last step (diagnostic / tests)
+        if self.offset_nerf_grad:
+            self.grad_vworld = torch.zeros(V, 3, device=dev)              # colour-field path, world space, loss-scaled
         if self.refine:
             # triangles_errors / triangles_errors_cnt (renderer.py:163-164): summed per-pixel loss and pixel count per face
             self.face_errors = torch.zeros(Fn, device=dev); self.face_counts = torch.zeros(Fn, device=dev)
@@ -188,6 +200,13 @@ class Stage1Trainer:
              ptr(self.denc_tiles), ptr(t0.g_mlp), ptr(t0.opt_state), 0, 1, stream())
         call("n2m_s0_encode_bwd", self._pp(), ptr(self.recs), ptr(self.counters), self.cap, ptr(self.pts), ptr(self.pdirs),
              ptr(self.denc_tiles), ptr(t0.table), ptr(t0.offsets), ptr(t0.gtables[t0.parity]), ptr(t0.opt_state), 0, 1, stream())
+        if self.offset_nerf_grad:
+            # d loss / d xyzs of every point (colour-net input + colour-grid input gradient, through contract()) -> the vertices, through
+            # dr.interpolate (grad_vworld) and dr.rasterize's (u, v) (grad_vclip, beside the antialias gradient)
+            self.grad_vworld.zero_()
+            call("n2m_s1_offset_grad", self._pp(), ptr(self.rast), ptr(self.vertices), ptr(self.vclip), ptr(self.triangles), ptr(self.inv),
+                 self.h, self.w, ptr(self.pts), ptr(self.denc_tiles), ptr(t0.table), ptr(t0.offsets), ptr(self.grad_vclip),
+                 ptr(self.grad_vworld), ptr(t0.opt_state), stream())
 
     def step(self, mvp, rays_d, gt, bg, shading="full", lr=None, use_graph=False):
         """One optimizer step on one view: mvp [4,4], rays_d [h0*w0,3] (unnormalised), gt [h0*w0, 3 or 4], bg [h0*w0,3].
@@ -233,16 +252,24 @@ class Stage1Trainer:
         th = self.topology
         if self.lambda_offsets > 0:
             self.loss_acc[0:1].add_(self.lambda_offsets * (self.offsets * self.offsets).sum(1).mean())          # utils.py:764-776
-        call("n2m_s1_vert_step", ptr(self.grad_vclip), ptr(self.mvp), ptr(th.keys), th.slots, ptr(self.base_vertices), ptr(self.offsets),
-             ptr(self.m_vert), ptr(self.v_vert), ptr(self.vertices), ptr(self.vert_scratch), ptr(self.grad_offsets), V, self.lambda_lap,
-             self.lambda_offsets, -1.0, self.t0.cfg.eps, ptr(self.t0.opt_state), ptr(self.vert_state), ptr(self.loss_acc), stream())
+        rest = (ptr(self.mvp), ptr(th.keys), th.slots, ptr(self.base_vertices), ptr(self.offsets), ptr(self.m_vert), ptr(self.v_vert),
+                ptr(self.vertices), ptr(self.vert_scratch), ptr(self.grad_offsets), V, self.lambda_lap, self.lambda_offsets, -1.0,
+                self.t0.cfg.eps, ptr(self.t0.opt_state), ptr(self.vert_state), ptr(self.loss_acc), stream())
+        if self.offset_nerf_grad:
+            call("n2m_s1_vert_step_world", ptr(self.grad_vclip), ptr(self.grad_vworld), *rest)
+        else:
+            call("n2m_s1_vert_step", ptr(self.grad_vclip), *rest)
 
     def vertex_gradient(self):
-        """d loss / d vertices [V,3] of the last `loss_backward` (through dr.antialias and the projection of renderer.py:858; the
-        gradient the reference accumulates on `vertices_offsets`), unscaled.  Valid when the step's found_inf flag is clear."""
+        """d loss / d vertices [V,3] of the last `loss_backward` (through dr.antialias and the projection of renderer.py:858, plus with
+        offset_nerf_grad the colour-field path through dr.interpolate / dr.rasterize; the gradient the reference accumulates on
+        `vertices_offsets`), unscaled.  Valid when the step's found_inf flag is clear."""
         if not self.antialias:
             raise RuntimeError("vertex gradients flow through dr.antialias only: construct Stage1Trainer(antialias=True)")
-        return (self.grad_vclip @ self.mvp[:, :3]) / self.t0.opt_state[0]
+        g = self.grad_vclip @ self.mvp[:, :3]
+        if self.offset_nerf_grad:
+            g = g + self.grad_vworld
+        return g / self.t0.opt_state[0]
 
     def read_loss(self):
         return float(self.loss_acc[0].item())

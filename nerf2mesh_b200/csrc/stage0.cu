@@ -406,7 +406,7 @@ encode_bwd_visit(const n2m_s0_params& p, const float4* __restrict__ recs,
 }
 
 // grid-stride over the (level group, tile) items of the part's range [lo, hi), group-major (see "Level-group walk" above); the
-// host sizes the grid to the CTAs that fit on the device at once
+// host sizes the grid to no more CTAs than fit on the device at once (encode_bwd_grid)
 template <bool SCATTER, bool TV>
 __global__ void __launch_bounds__(kTile)
 k_s0_encode_bwd(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* __restrict__ counters,
@@ -746,8 +746,13 @@ static inline uint32_t part_grid(uint32_t Mcap, uint32_t nparts) {
     return nparts <= 1 ? Mcap / kTile : div_up(Mcap / kTile, nparts) + 1;
 }
 
-// blocks for one scatter / TV launch: the CTAs that are resident on the device at once (read once per process), so that the
-// group-major item order is also the order in which the items run; never more than the launch has items
+// blocks for one scatter / TV launch: the CTAs that are resident on the device at once (read once per process), divided among the
+// `nparts` ray-range parts whose scatters the step runs side by side, so that the group-major item order is also the order in
+// which the items run; never more than the launch has items.
+// With a whole-device grid per part, the first part's CTAs hold every SM slot for their whole walk and the next part queues behind
+// them, so the level groups' slices of the gradient table are each filled and written back once per part.  Sharing the device,
+// the parts walk the groups side by side and meet in the same slice.  On an H100 80GB HBM3 (700 W) this took the two lego parts'
+// scatters from 428 to 394 us and the lego step from 1.176 to 1.131 ms.
 template <bool SCATTER, bool TV>
 static uint32_t encode_bwd_grid(uint32_t Mcap, uint32_t nparts) {
     static int per_sm = 0;
@@ -755,7 +760,7 @@ static uint32_t encode_bwd_grid(uint32_t Mcap, uint32_t nparts) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_s0_encode_bwd<SCATTER, TV>, kTile, 0);
         if (per_sm <= 0) per_sm = 1;
     }
-    return min((uint32_t)(per_sm * num_sms()), kLevelGroups * part_grid(Mcap, nparts));
+    return min(max(1u, (uint32_t)(per_sm * num_sms()) / nparts), kLevelGroups * part_grid(Mcap, nparts));
 }
 
 extern "C" {

@@ -67,7 +67,8 @@ typedef struct {
     uint32_t grid_size;
     uint32_t num_levels;    /* must be 16 */
     uint32_t base_res;
-    uint32_t shading_full;  /* 0 = 'diffuse' (first diffuse_step iterations), 1 = 'full' */
+    uint32_t shading_full;  /* 0 = 'diffuse' (first diffuse_step iterations), 1 = 'full'; 2 = 'specular': n2m_s0_mlp_fwd only (evaluation),
+                               which then writes (sigma, specular) -- the training and backward kernels take 0 or 1 */
     uint32_t gt_has_alpha;  /* gt is rgba: blend with bg and add the mask loss (utils.py:662-667,681-683) */
 } n2m_s0_params;
 

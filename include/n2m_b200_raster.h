@@ -89,6 +89,14 @@ int n2m_s1_loss_aa(const void* aa, const float* gt, uint32_t gt_channels, const 
                    n2m_stream_t stream);
 int n2m_s1_dout(const void* grad_rgba, const int32_t* inv, uint32_t num_pixels, void* dout, n2m_stream_t stream);
 
+/* evaluation (render_stage1 at inference, renderer.py:886-907): n2m_s1_render_compose, one thread per low-res pixel of h0 x w0, over
+ * img [h*w] float4 = (r, g, b, alpha) at (h, w) = ssaa * (h0, w0) -- the antialiased image, or n2m_s1_rgba's (alpha 0 or 1) --, and
+ * rast [h,w,4] of the same view: image [h0*w0,3] = mean(clamp(alpha) * clamp(rgb)) + (1 - mean(clamp(alpha))) * bg [h0*w0,3],
+ * weights_sum [h0*w0] = mean(clamp(alpha)), depth [h0*w0] = mean(clamp(alpha) * rast.z).  image and weights_sum are bit-identical to
+ * those n2m_s1_loss_aa writes for the same img (and n2m_s1_loss for the n2m_s1_rgba image); nothing else is written. */
+int n2m_s1_render_compose(const void* img, const float* rast, const float* bg, uint32_t h0, uint32_t w0, uint32_t ssaa, float* image,
+                          float* weights_sum, float* depth, n2m_stream_t stream);
+
 /* mesh refinement (opt.refine: update_triangles_errors, renderer.py:893-903,923-943; utils.py:720-721): n2m_s1_loss_err and
  * n2m_s1_loss_aa_err are n2m_s1_loss / n2m_s1_loss_aa that also, for every low-res pixel whose top-left super-sample (y0*ssaa, x0*ssaa)
  * of rast [h,w,4] is covered by face f (rast.w = f + 1, f < F), add the pixel's loss (before the 1/(h0*w0) mean and without loss_scale)

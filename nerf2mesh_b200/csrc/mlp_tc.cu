@@ -90,7 +90,8 @@ k_mlp_fwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const int32_t*
                                       tid, sp, sync_before_mma);
         const uint32_t j = tile * kTile + r;
         if (j >= pr.lo && j < pr.hi) {
-            out[j] = o;
+            // shading 'specular' (network.py:183-184, evaluation only): the colour is the specular term alone
+            out[j] = p.shading_full == 2 ? make_float4(o.x, sp[0], sp[1], sp[2]) : o;
             spec_sq += sp[0] * sp[0] + sp[1] * sp[1] + sp[2] * sp[2];
         }
         sync_before_mma();          // all reads of this tile's smem are done before the next bulk copy

@@ -25,6 +25,8 @@
 // and the vertex step becomes n2m_s1_vert_step_world.
 // With mesh refinement on (opt.refine), n2m_s1_loss_err / n2m_s1_loss_aa_err replace the two loss launches: the same kernels, which also
 // accumulate each pixel's loss and a hit into the face it sees (update_triangles_errors, renderer.py:893-903,923-943; utils.py:720-721).
+// Evaluation (render_stage1 at inference: eval_step / test_step, utils.py:853,882) runs the forward part of the step and then
+//   n2m_s1_render_compose             clamp, alphas * rgbs, ssaa average, background mix, weights_sum and depth -- no gt, no loss, no gradient
 #include "n2m_common.cuh"
 #include "raster_grad.cuh"
 #include "s0_geom.cuh"
@@ -260,6 +262,36 @@ k_s1_loss_aa(const float4* __restrict__ aa, const float* __restrict__ gt, uint32
         for (int i = 0; i < 8; ++i) s += red[i];
         atomicAdd(loss_out, s);
     }
+}
+
+// ---- evaluation (render_stage1 at inference, renderer.py:886-907): the image part of k_s1_loss_aa, plus depth ----
+// One thread per low-resolution pixel over img [h*w] float4 = (r, g, b, alpha), antialiased or the n2m_s1_rgba image (alpha exactly 0 or
+// 1).  The float operations are those of k_s1_loss_aa in the same order, so image / weights_sum equal its outputs bit for bit; on the
+// n2m_s1_rgba image they also equal k_s1_loss's (al = 1: al * c == c; al = 0 adds +0 to a non-negative sum).  depth = mean over the
+// super-samples of alpha * rast.z (z/w; :889,:900).
+__global__ void __launch_bounds__(256)
+k_s1_render_compose(const float4* __restrict__ img, const float4* __restrict__ rast, const float* __restrict__ bg, uint32_t h0, uint32_t w0,
+                    uint32_t ssaa, float* __restrict__ image, float* __restrict__ weights_sum, float* __restrict__ depth) {
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= h0 * w0) return;
+    const uint32_t y0 = q / w0, x0 = q % w0, w = w0 * ssaa;
+    const float inv_s2 = 1.0f / (float)(ssaa * ssaa);
+    float r = 0.f, g = 0.f, b = 0.f, a = 0.f, d = 0.f;
+    for (uint32_t dy = 0; dy < ssaa; ++dy)
+        for (uint32_t dx = 0; dx < ssaa; ++dx) {
+            const size_t i = (size_t)(y0 * ssaa + dy) * w + x0 * ssaa + dx;
+            const float4 v = img[i];
+            const float al = clampf(v.w, 0.f, 1.f);
+            r += al * clampf(v.x, 0.f, 1.f); g += al * clampf(v.y, 0.f, 1.f); b += al * clampf(v.z, 0.f, 1.f); a += al;
+            d += al * rast[i].z;
+        }
+    r *= inv_s2; g *= inv_s2; b *= inv_s2; a *= inv_s2; d *= inv_s2;
+    const float T = 1.f - a;
+    const float b0 = bg[3 * q], b1 = bg[3 * q + 1], b2 = bg[3 * q + 2];
+    const float pr = r + T * b0, pg = g + T * b1, pb = b + T * b2;
+    image[3 * q] = pr; image[3 * q + 1] = pg; image[3 * q + 2] = pb;
+    weights_sum[q] = a;
+    depth[q] = d;
 }
 
 // ---- colour-field path of the vertex gradient (--enable_offset_nerf_grad: renderer.py:877-879 with xyzs[mask_flatten] not detached) ----
@@ -528,6 +560,16 @@ int n2m_s1_loss_aa_err(const void* aa, const float* gt, uint32_t gt_channels, co
                        const float* rast, float* face_err, float* face_cnt, uint32_t F, n2m_stream_t stream) {
     return launch_s1_loss_aa<true>(aa, gt, gt_channels, bg, h0, w0, ssaa, lambda_mask, loss_scale, d_aa, image, weights_sum, loss_out,
                                    rast, face_err, face_cnt, F, stream, "s1_loss_aa_err");
+}
+
+int n2m_s1_render_compose(const void* img, const float* rast, const float* bg, uint32_t h0, uint32_t w0, uint32_t ssaa, float* image,
+                          float* weights_sum, float* depth, n2m_stream_t stream) {
+    N2M_REQUIRE(img && rast && bg && image && weights_sum && depth, "s1_render_compose", "null pointer");
+    N2M_REQUIRE(ssaa >= 1, "s1_render_compose", "ssaa must be >= 1");
+    if (h0 == 0 || w0 == 0) return 0;
+    k_s1_render_compose<<<div_up(h0 * w0, 256u), 256, 0, as_stream(stream)>>>(static_cast<const float4*>(img), reinterpret_cast<const float4*>(rast),
+                                                                             bg, h0, w0, ssaa, image, weights_sum, depth);
+    return check_launch("s1_render_compose");
 }
 
 int n2m_s1_vert_check(const float* grad_vclip, uint32_t V, float* opt_state, n2m_stream_t stream) {

@@ -7,6 +7,8 @@
 //                          and scattered into the full-resolution feature image (renderer.py:349-376)
 //   n2m_s1_inpaint         gutter inpaint (renderer.py:378-394): morphological classification + exact windowed nearest-neighbour search
 //   n2m_s1_ssaa_down2      the 2x down-sample (cv2.resize INTER_LINEAR at half size, renderer.py:400-402) and the channel split
+// and the viewer's side of the export (renderer.html:54-160):
+//   n2m_s1_asset_shade     the fragment shader on the rasterized asset: nearest texel of feat0 / feat1, specular_net in fp32, modes
 #include "n2m_common.cuh"
 #include "mlp_common.cuh"
 #include "../../include/n2m_b200_texture.h"
@@ -247,6 +249,79 @@ k_ssaa_down2(const uint8_t* __restrict__ feats, uint32_t h0, uint32_t w0, uint32
     for (int c = 0; c < 3; ++c) { feat0[(size_t)q * 3 + c] = out[c]; feat1[(size_t)q * 3 + c] = out[3 + c]; }
 }
 
+// ================================================================================================
+// the exported asset as the viewer draws it (renderer.html:54-160, textures :441-450)
+// ================================================================================================
+constexpr int kSpecIn = 6, kSpecHidden = 32, kSpecOut = 3, kSpecWeights = kSpecHidden * kSpecIn + kSpecOut * kSpecHidden;
+
+// u * a0 + v * a1 + (1 - u - v) * a2 with every product and sum rounded on its own (no contraction), so a float32 restatement of the
+// expression gives the same bits and the same nearest texel
+__device__ __forceinline__ float bary_rn(float u, float v, float ww, float a0, float a1, float a2) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(u, a0), __fmul_rn(v, a1)), __fmul_rn(ww, a2));
+}
+
+// nearest texel of an RGB uint8 texture [H,W,3] at (s, t), three.js NearestFilter + flipY + clamp-to-edge
+__device__ __forceinline__ const uint8_t* nearest_texel(const uint8_t* tex, int H, int W, float s, float t) {
+    const int x = min(max((int)floorf(__fmul_rn(s, (float)W)), 0), W - 1);
+    const int y = min(max(H - 1 - (int)floorf(__fmul_rn(t, (float)H)), 0), H - 1);
+    return tex + ((size_t)y * W + x) * 3;
+}
+
+// one thread per super-sample: covered ones -> (r, g, b, 1), the others -> 0
+__global__ void __launch_bounds__(256)
+k_s1_asset_shade(const float4* __restrict__ rast, uint32_t n, const float* __restrict__ verts, const int32_t* __restrict__ tri,
+                 const float* __restrict__ st, const int32_t* __restrict__ ft, const int32_t* __restrict__ face_offsets, uint32_t cascades,
+                 const uint8_t* const* __restrict__ feat0, const uint8_t* const* __restrict__ feat1, const int32_t* __restrict__ tex_size,
+                 const float* __restrict__ mlp, float cx, float cy, float cz, uint32_t mode, float4* __restrict__ img) {
+    __shared__ float sw[kSpecWeights];
+    for (int k = threadIdx.x; k < kSpecWeights; k += blockDim.x) sw[k] = mlp[k];
+    __syncthreads();
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float4 r = rast[i];
+    if (!(r.w > 0.f)) { img[i] = make_float4(0.f, 0.f, 0.f, 0.f); return; }
+    const int32_t f = (int32_t)r.w - 1;
+    uint32_t c = 0;
+    while (c + 1 < cascades && f >= face_offsets[c + 1]) ++c;
+    const float u = r.x, v = r.y, ww = __fsub_rn(__fsub_rn(1.f, r.x), r.y);
+    const int t0 = ft[3 * f], t1 = ft[3 * f + 1], t2 = ft[3 * f + 2];
+    const float s = bary_rn(u, v, ww, st[2 * t0], st[2 * t1], st[2 * t2]);
+    const float t = bary_rn(u, v, ww, st[2 * t0 + 1], st[2 * t1 + 1], st[2 * t2 + 1]);
+    const int H = tex_size[2 * c], W = tex_size[2 * c + 1];
+    const uint8_t* d = nearest_texel(feat0[c], H, W, s, t);
+    float rgb[3] = {d[0] / 255.f, d[1] / 255.f, d[2] / 255.f};
+    if (mode != 1) {
+        const int i0 = tri[3 * f], i1 = tri[3 * f + 1], i2 = tri[3 * f + 2];
+        const float cam[3] = {cx, cy, cz};
+        float x[kSpecIn];
+#pragma unroll
+        for (int a = 0; a < 3; ++a)
+            x[a] = bary_rn(u, v, ww, verts[3 * (size_t)i0 + a], verts[3 * (size_t)i1 + a], verts[3 * (size_t)i2 + a]) - cam[a];
+        const float inv_len = 1.f / sqrtf(x[0] * x[0] + x[1] * x[1] + x[2] * x[2]);        // normalize(rayDirection)
+#pragma unroll
+        for (int a = 0; a < 3; ++a) x[a] *= inv_len;
+        const uint8_t* p = nearest_texel(feat1[c], H, W, s, t);
+#pragma unroll
+        for (int a = 0; a < 3; ++a) x[3 + a] = p[a] / 255.f;
+        float o[kSpecOut] = {0.f, 0.f, 0.f};
+#pragma unroll 4
+        for (int j = 0; j < kSpecHidden; ++j) {
+            float hj = 0.f;
+#pragma unroll
+            for (int k = 0; k < kSpecIn; ++k) hj += sw[j * kSpecIn + k] * x[k];
+            hj = fmaxf(hj, 0.f);
+#pragma unroll
+            for (int q = 0; q < kSpecOut; ++q) o[q] += sw[kSpecHidden * kSpecIn + q * kSpecHidden + j] * hj;
+        }
+#pragma unroll
+        for (int q = 0; q < kSpecOut; ++q) {
+            const float spec = 1.f / (1.f + expf(-o[q]));
+            rgb[q] = mode == 2 ? spec : fminf(fmaxf(rgb[q] + spec, 0.f), 1.f);
+        }
+    }
+    img[i] = make_float4(rgb[0], rgb[1], rgb[2], 1.f);
+}
+
 }  // namespace
 }  // namespace n2m
 
@@ -310,6 +385,20 @@ int n2m_s1_ssaa_down2(const uint8_t* feats, uint32_t h0, uint32_t w0, uint32_t s
     if (h0 == 0 || w0 == 0) return 0;
     k_ssaa_down2<<<div_up(h0 * w0, 256u), 256, 0, as_stream(stream)>>>(feats, h0, w0, ssaa, feat0, feat1);
     return check_launch("s1_ssaa_down2");
+}
+
+int n2m_s1_asset_shade(const float* rast, uint32_t num_pixels, const float* verts, const int32_t* tri, const float* st, const int32_t* ft,
+                       const int32_t* face_offsets, uint32_t cascades, const void* const* feat0, const void* const* feat1, const int32_t* tex_size,
+                       const float* mlp, float cam_x, float cam_y, float cam_z, uint32_t mode, float* img, n2m_stream_t stream) {
+    N2M_REQUIRE(rast && verts && tri && st && ft && face_offsets && feat0 && feat1 && tex_size && mlp && img, "s1_asset_shade", "null pointer");
+    N2M_REQUIRE(cascades >= 1, "s1_asset_shade", "at least one cascade");
+    N2M_REQUIRE(mode >= 1 && mode <= 3, "s1_asset_shade", "mode must be 1 (diffuse), 2 (specular) or 3 (full)");
+    if (num_pixels == 0) return 0;
+    k_s1_asset_shade<<<div_up(num_pixels, 256u), 256, 0, as_stream(stream)>>>(
+        reinterpret_cast<const float4*>(rast), num_pixels, verts, tri, st, ft, face_offsets, cascades,
+        reinterpret_cast<const uint8_t* const*>(feat0), reinterpret_cast<const uint8_t* const*>(feat1), tex_size, mlp, cam_x, cam_y, cam_z, mode,
+        reinterpret_cast<float4*>(img));
+    return check_launch("s1_asset_shade");
 }
 
 }  // extern "C"

@@ -25,7 +25,9 @@ Unbounded scenes (bound > 1): `vertices` / `triangles` may be equal-length lists
 trainer concatenates with index offsets as the reference does (renderer.py:130-157, `v_cumsum` / `f_cumsum`); every kernel of the step then
 runs on the concatenated mesh, and `cascade_mesh(cas)` returns one cascade for the export.  Refinement looks at cascade 0 only
 (renderer.py:223-225) and `replace_mesh` replaces cascade 0, rebasing the outer cascades on their current vertices (:258-285).  With
-Stage0Config(contract=True) the surface points are contracted before the colour field is queried (n2m_s1_points_contract).  Not built: the
+Stage0Config(contract=True) the surface points are contracted before the colour field is queried (n2m_s1_points_contract).
+`render()` is render_stage1 at inference (eval_step / test_step, utils.py:853,882): the forward part of the step on buffers of its own, then
+n2m_s1_render_compose -> image, weights_sum, depth, in shading 'diffuse', 'specular' or 'full'.  Not built: the
 pytorch3d regularisers that are off by default (lambda_normal, lambda_edgelen) and SDF mode's all-ones refinement mask.
 """
 import ctypes
@@ -51,7 +53,21 @@ _lib.register({
     "n2m_s1_vert_step": [P, P, P, U, P, P, P, P, P, P, P, U, F, F, F, F, P, P, P, P],
     "n2m_s1_offset_grad": [P, P, P, P, P, P, U, U, P, P, P, P, P, P, P, P],
     "n2m_s1_vert_step_world": [P, P, P, P, U, P, P, P, P, P, P, P, U, F, F, F, F, P, P, P, P],
+    "n2m_s1_render_compose": [P, P, P, U, U, U, P, P, P, P],
 })
+
+# shading -> n2m_s0_params.shading_full of the forward MLP launch ('specular': the specular term alone, evaluation only)
+SHADING_MODES = {"diffuse": 0, "full": 1, "specular": 2}
+
+
+def bg_image(bg_color, q, device):
+    """bg_color (a scalar, or a tensor [q,3]) as the contiguous float32 [q,3] device tensor the compose kernel reads"""
+    if torch.is_tensor(bg_color):
+        bg = bg_color.to(device, torch.float32).reshape(-1, 3).contiguous()
+        if bg.shape[0] != q:
+            raise ValueError(f"bg_color: {bg.shape[0]} rows for {q} pixels")
+        return bg
+    return torch.full((q, 3), float(bg_color), device=device)
 
 
 class Stage1Trainer:
@@ -89,6 +105,7 @@ class Stage1Trainer:
         self.vclip = None
         self.mvp = None
         self._graphs, self._warm = {}, False
+        self._render_cache, self._render_th = {}, None       # render(): buffers per (h0, w0), the edge hash of a non-antialiased trainer
         # vertex offsets (main.py:49,84-85 defaults: lr_vert 1e-4, lambda_lap 1e-3, lambda_offsets 0.1); 0 = vertices fixed
         self.lr_vert, self.lambda_lap, self.lambda_offsets = float(lr_vert), float(lambda_lap), float(lambda_offsets)
         if self.lr_vert > 0:
@@ -155,6 +172,8 @@ class Stage1Trainer:
     def forward(self, mvp, rays_d, shading="full"):
         """rasterize -> surface points -> colour MLPs; leaves per-point colours in `out`, the pixel -> point map in `inv`."""
         t0 = self.t0
+        if shading == "specular":
+            raise ValueError("shading 'specular' is for render() only: the step trains with 'diffuse' or 'full'")
         self.params.shading_full = int(shading == "full")
         mvp = mvp.to(t0.device, torch.float32).contiguous()
         vclip = (torch.nn.functional.pad(self.vertices, (0, 1), value=1.0) @ mvp.T).contiguous()           # renderer.py:858
@@ -273,6 +292,82 @@ class Stage1Trainer:
 
     def read_loss(self):
         return float(self.loss_acc[0].item())
+
+    @torch.no_grad()
+    def render(self, mvp, rays_d, h0=None, w0=None, bg_color=1.0, shading="full", antialias=True):
+        """render_stage1 at inference (renderer.py:816-921; eval_step / test_step, utils.py:853,882): mvp [4,4], rays_d [h0*w0,3] (the
+        low-res per-pixel directions, unnormalised, as step() takes them), bg_color a scalar or [h0*w0,3], shading 'diffuse' / 'specular' /
+        'full'.  Returns (image [h0*w0,3], weights_sum [h0*w0], depth [h0*w0]) on the device; depth is the mean over the super-samples of
+        alpha * z/w (:889,:900).  h0, w0 default to the trainer's; any other resolution works.
+
+        The pipeline of forward() at ssaa * (h0, w0) -- rasterize, surface points (contracted when cfg.contract), gather, colour MLPs,
+        with `antialias` (the reference always antialiases here) n2m_s1_rgba + dr.antialias -- then n2m_s1_render_compose.  It runs on
+        buffers of its own per (h0, w0), with a point cap of every super-sample, and leaves the step's buffers, the optimizer state and the
+        captured step graphs untouched.  The EMA is the caller's: t0.ema_apply() / t0.ema_restore() around the call."""
+        if shading not in SHADING_MODES:
+            raise ValueError(f"shading must be one of {sorted(SHADING_MODES)}")
+        t0 = self.t0
+        dev = t0.device
+        h0 = self.h0 if h0 is None else int(h0)
+        w0 = self.w0 if w0 is None else int(w0)
+        Q = h0 * w0
+        rays_d = rays_d.to(dev, torch.float32).contiguous()
+        if tuple(rays_d.shape) != (Q, 3):
+            raise ValueError(f"rays_d must be [{Q},3] for a {h0}x{w0} render")
+        bg = bg_image(bg_color, Q, dev)
+        rb = self._render_buffers(h0, w0)
+        h, w = rb["h"], rb["w"]
+        params = type(self.params)()
+        ctypes.memmove(ctypes.byref(params), ctypes.byref(self.params), ctypes.sizeof(params))
+        params.shading_full = SHADING_MODES[shading]
+        pp = ctypes.byref(params)
+        mvp = mvp.to(dev, torch.float32).contiguous()
+        vclip = (torch.nn.functional.pad(self.vertices, (0, 1), value=1.0) @ mvp.T).contiguous()            # as forward()
+        rast, _ = dr.rasterize(rb["glctx"], vclip[None], self.triangles, (h, w))
+        rb["rast"] = rast
+        call("n2m_s1_points_contract", ptr(rast), ptr(self.vertices), ptr(self.triangles), ptr(rays_d), h, w, self.ssaa, rb["cap"],
+             ptr(rb["counters"]), ptr(rb["inv"]), ptr(rb["pts"]), ptr(rb["pdirs"]), ptr(rb["recs"]), int(self.contract), stream())
+        call("n2m_s0_encode_points", pp, ptr(rb["pts"]), ptr(rb["pdirs"]), ptr(rb["counters"]), rb["cap"], ptr(t0.table), ptr(t0.offsets),
+             ptr(rb["enc_tiles"]), stream())
+        call("n2m_s0_mlp_fwd", pp, ptr(rb["enc_tiles"]), ptr(rb["counters"]), rb["cap"], ptr(t0.wpack), ptr(rb["out"]), None, 0, 1, stream())
+        call("n2m_s1_rgba", ptr(rb["out"]), ptr(rb["inv"]), h * w, ptr(rb["rgba"]), stream())
+        img = rb["rgba"]
+        if antialias:
+            th = self._render_topology()
+            if "aa" not in rb:
+                rb["aa"] = torch.empty(h * w, 4, device=dev)
+            call("n2m_antialias_forward", ptr(rb["rgba"]), ptr(rast), ptr(vclip), ptr(self.triangles), ptr(th.keys), ptr(th.opp), th.slots,
+                 h, w, 4, ptr(rb["aa"]), stream())
+            img = rb["aa"]
+        image = torch.empty(Q, 3, device=dev); weights_sum = torch.empty(Q, device=dev); depth = torch.empty(Q, device=dev)
+        call("n2m_s1_render_compose", ptr(img), ptr(rast), ptr(bg), h0, w0, self.ssaa, ptr(image), ptr(weights_sum), ptr(depth), stream())
+        return image, weights_sum, depth
+
+    def _render_buffers(self, h0, w0):
+        """render()'s buffers for a (h0, w0) render, made on first use and cached: its own rasterizer scratch (the step's graphs hold the
+        addresses of the trainer's), point buffers with room for every super-sample, the (r, g, b, alpha) image"""
+        rb = self._render_cache.get((h0, w0))
+        if rb is None:
+            dev = self.t0.device
+            h, w = h0 * self.ssaa, w0 * self.ssaa
+            n = h * w
+            cap = (n + 127) // 128 * 128
+            rb = self._render_cache[(h0, w0)] = dict(
+                h=h, w=w, cap=cap, glctx=dr.RasterizeCudaContext(dev), inv=torch.empty(n, dtype=torch.int32, device=dev),
+                pts=torch.zeros(cap, 3, device=dev), pdirs=torch.zeros(cap, 3, device=dev), recs=torch.zeros(cap, 4, device=dev),
+                counters=torch.zeros(16, dtype=torch.int32, device=dev), enc_tiles=torch.zeros(cap * 64, dtype=torch.float16, device=dev),
+                out=torch.zeros(cap, 4, device=dev), rgba=torch.empty(n, 4, device=dev))
+        return rb
+
+    def _render_topology(self):
+        """the edge hash of the current mesh for render()'s antialias: the step's when it antialiases, else one built on first use (and
+        again after replace_mesh)"""
+        if self.antialias:
+            return self.topology
+        th = self._render_th
+        if th is None or th.tri is not self.triangles:
+            th = self._render_th = dr.TopologyHash(self.triangles)
+        return th
 
     def refine_mask(self):
         """refine_and_decimate's face mask (renderer.py:217-240, not SDF) over the faces of cascade 0 (:223-225; with one mesh, all faces):

@@ -16,6 +16,13 @@ The stages, each callable on its own:
 
 Everything up to the JPEG encode stays on the device; the only host copies are the two finished textures.  A mesh that covers no texel
 gives zero textures (the reference fails in its nearest-neighbour fit there).
+
+Looking at the result -- what the viewer (renderer.html) shows, and how much the bake loses against Stage1Trainer.render:
+    asset = load_exported(save_path)                                      # the files: OBJ, JPEGs (BGR -> RGB), mlp.json
+    asset = ExportedMesh.from_export(s1, vt, ft, feats)                   # the same from export_stage1's return value, before the JPEG
+    image, weights_sum, depth = render_exported(asset, mvp, campos, h0, w0, ssaa=1, shading="full", antialias=False)
+render_exported rasterizes every cascade into one depth buffer and runs the viewer's fragment shader on the device (n2m_s1_asset_shade:
+nearest texel, specular_net in fp32), then the evaluation compose of Stage1Trainer.render.
 """
 import json
 import os
@@ -26,13 +33,14 @@ import torch
 from . import _lib
 from . import raster as dr
 from . import stage0  # noqa: F401  (binds the stage-0 gather n2m_s0_encode_points)
-from ._lib import P, U, call, ptr, stream
+from ._lib import F, P, U, call, ptr, stream
 
 _lib.register({
     "n2m_s1_bake_points": [P, P, P, U, U, U, U, U, P, P, P, P],
     "n2m_s1_geo_feat": [P, P, U, P, P, P, P, P],
     "n2m_s1_inpaint": [P, P, U, U, P, P, P],
     "n2m_s1_ssaa_down2": [P, U, U, U, P, P, P],
+    "n2m_s1_asset_shade": [P, U, P, P, P, P, P, U, P, P, P, P, F, F, F, U, P, P],
 })
 
 MAX_BAND_POINTS = 1 << 22          # points per band: 512 MiB of gather tiles (128 B per point) + 64 MiB of positions and texel indices
@@ -258,3 +266,148 @@ def export_stage1(s1, save_path, vt, ft, resolution=4096, band_rows=None):
         feats.append((feat0, feat1))
     write_mlp_json(os.path.join(save_path, "mlp.json"), specular_weights(t0), bound=t0.cfg.bound, cascade=C)
     return feats if per_cascade else feats[0]
+
+
+# ---- the exported asset, rendered as the viewer draws it -----------------------------------------------------------------------------
+SHADE_MODES = {"diffuse": 1, "specular": 2, "full": 3}          # the viewer's `mode` uniform (renderer.html:148-158)
+
+
+class ExportedMesh:
+    """The textured mesh of an export on the device, every cascade concatenated as the viewer draws them into one depth buffer:
+    vertices [V,3] float32, triangles [F,3] int32 (indices into the concatenated vertices), st [Nt,2] float32 = the OBJ's texture
+    coordinates (s, t) with t = 1 - v as written, ft [F,3] int32 (into the concatenated st), face_offsets [C+1] (host ints; cascade c owns
+    faces face_offsets[c] .. face_offsets[c+1]-1), feat0 / feat1 [C] lists of RGB uint8 [H_c,W_c,3] textures, weights
+    {net.0.weight [32,6], net.1.weight [3,32]} float32 ([out, in]), bound."""
+
+    def __init__(self, vertices, triangles, st, ft, feat0, feat1, weights, bound=1.0, device="cuda"):
+        C = len(vertices)
+        if not (len(triangles) == len(st) == len(ft) == len(feat0) == len(feat1) == C and C > 0):
+            raise ValueError("ExportedMesh: one (vertices, triangles, st, ft, feat0, feat1) per cascade")
+        dev = torch.device(device)
+        vs, fs, sts, fts, self.face_offsets = [], [], [], [], [0]
+        v_off = t_off = 0
+        for v, f, s, t in zip(vertices, triangles, st, ft):
+            v = _np(v, np.float32); s = _np(s, np.float32)
+            f = _np(f, np.int64); t = _np(t, np.int64)
+            if f.shape != t.shape:
+                raise ValueError("ExportedMesh: ft must match triangles row for row")
+            vs.append(v); sts.append(s); fs.append(f + v_off); fts.append(t + t_off)
+            v_off += v.shape[0]; t_off += s.shape[0]
+            self.face_offsets.append(self.face_offsets[-1] + f.shape[0])
+        self.vertices = torch.from_numpy(np.concatenate(vs)).to(dev).contiguous()
+        self.triangles = torch.from_numpy(np.concatenate(fs).astype(np.int32)).to(dev).contiguous()
+        self.st = torch.from_numpy(np.concatenate(sts)).to(dev).contiguous()
+        self.ft = torch.from_numpy(np.concatenate(fts).astype(np.int32)).to(dev).contiguous()
+        self.feat0 = [_as_tensor(x, torch.uint8, dev) for x in feat0]
+        self.feat1 = [_as_tensor(x, torch.uint8, dev) for x in feat1]
+        for a, b in zip(self.feat0, self.feat1):
+            if a.dim() != 3 or a.shape[2] != 3 or a.shape != b.shape:
+                raise ValueError("ExportedMesh: feat0 / feat1 of a cascade must both be [H,W,3]")
+        self.weights = {k: _np(weights[k], np.float32) for k in ("net.0.weight", "net.1.weight")}
+        if self.weights["net.0.weight"].shape != (32, 6) or self.weights["net.1.weight"].shape != (3, 32):
+            raise ValueError("ExportedMesh: specular_net weights must be [32,6] and [3,32]")
+        self.bound = float(bound)
+        # the kernel's view of it: face offsets, texture pointers and sizes, the MLP weights, on the device
+        self._offsets = torch.tensor(self.face_offsets, dtype=torch.int32, device=dev)
+        self._feat0_ptrs = torch.tensor([t.data_ptr() for t in self.feat0], dtype=torch.int64, device=dev)
+        self._feat1_ptrs = torch.tensor([t.data_ptr() for t in self.feat1], dtype=torch.int64, device=dev)
+        self._tex_size = torch.tensor([[t.shape[0], t.shape[1]] for t in self.feat0], dtype=torch.int32, device=dev)
+        self._mlp = torch.from_numpy(np.concatenate([self.weights["net.0.weight"].ravel(), self.weights["net.1.weight"].ravel()])).to(dev)
+        self._topology = None
+
+    @property
+    def cascades(self):
+        return len(self.feat0)
+
+    def topology(self):
+        """the edge hash of the concatenated mesh (antialias), built on first use"""
+        if self._topology is None:
+            self._topology = dr.TopologyHash(self.triangles)
+        return self._topology
+
+    @classmethod
+    def from_export(cls, s1, vt, ft, feats):
+        """The asset export_stage1(s1, ..., vt, ft) writes, from its in-memory results: `feats` is its return value ((feat0, feat1), or a
+        list of them per cascade, with vt / ft lists), the mesh is s1.cascade_mesh(cas), the weights are the trainer's.  The texture
+        coordinates are the file's, t = float32(1 - v); the textures are the ones before the JPEG encode."""
+        per_cascade = isinstance(vt, (list, tuple))
+        vts, fts = (list(vt), list(ft)) if per_cascade else ([vt], [ft])
+        feats = list(feats) if per_cascade else [feats]
+        meshes = [s1.cascade_mesh(cas) for cas in range(s1.cascades)]
+        st = []
+        for x in vts:
+            x = _np(x, np.float32)
+            st.append(np.stack([x[:, 0], np.float32(1) - x[:, 1]], axis=1).astype(np.float32))          # write_obj's float32 expression
+        return cls([v for v, _ in meshes], [f for _, f in meshes], st, fts, [a for a, _ in feats], [b for _, b in feats],
+                   specular_weights(s1.t0), bound=s1.t0.cfg.bound, device=s1.t0.device)
+
+
+def read_obj(path):
+    """(v [V,3] float32, st [Nt,2] float32, f [F,3] int64, ft [F,3] int64; 0-based) of an OBJ in write_obj's layout: the `v` lines, the `vt`
+    lines, `usemtl`, the `f a/at b/bt c/ct` lines -- parsed block by block with numpy, the %.9g floats back to the float32 values written."""
+    with open(path) as fp:
+        text = fp.read()
+    a, b, c = text.find("\nv "), text.find("\nvt "), text.find("\nf ")
+    if min(a, b, c) < 0 or not a < b < c:
+        raise ValueError(f"{path}: not an OBJ in the layout write_obj writes (v, vt, then f lines)")
+    v = np.array(text[a:b].split()).reshape(-1, 4)[:, 1:].astype(np.float32)
+    vt_block = text[b:text.find("\nusemtl", b)] if text.find("\nusemtl", b) >= 0 else text[b:c]
+    st = np.array(vt_block.split()).reshape(-1, 3)[:, 1:].astype(np.float32)
+    faces = np.array(text[c:].replace("/", " ").split()).reshape(-1, 7)[:, 1:].astype(np.int64) - 1
+    return v, st, faces[:, 0::2], faces[:, 1::2]
+
+
+def load_exported(path, device="cuda"):
+    """The asset export_stage1 wrote under `path`: mlp.json (the specular_net weights, stored [in, out], transposed back; bound; the
+    cascade count), mesh_{cas}.obj and feat0_{cas}.jpg / feat1_{cas}.jpg (cv2.imread, BGR -> RGB) for every cascade -> ExportedMesh."""
+    import cv2
+    with open(os.path.join(path, "mlp.json")) as fp:
+        mlp = json.load(fp)
+    weights = {k: np.asarray(mlp[k], dtype=np.float32).T for k in ("net.0.weight", "net.1.weight")}
+    vs, fs, sts, fts, f0s, f1s = [], [], [], [], [], []
+    for cas in range(int(mlp["cascade"])):
+        v, st, f, ft = read_obj(os.path.join(path, f"mesh_{cas}.obj"))
+        vs.append(v); sts.append(st); fs.append(f); fts.append(ft)
+        for name, out in ((f"feat0_{cas}.jpg", f0s), (f"feat1_{cas}.jpg", f1s)):
+            img = cv2.imread(os.path.join(path, name))
+            if img is None:
+                raise FileNotFoundError(os.path.join(path, name))
+            out.append(np.ascontiguousarray(img[..., ::-1]))
+    return ExportedMesh(vs, fs, sts, fts, f0s, f1s, weights, bound=mlp["bound"], device=device)
+
+
+@torch.no_grad()
+def render_exported(asset, mvp, campos, h0, w0, ssaa=1, bg_color=1.0, shading="full", antialias=False, glctx=None):
+    """The asset as the viewer draws it (renderer.html:54-160): all cascades rasterized together at ssaa * (h0, w0) with the clip-space
+    transform mvp [4,4] (nvdiffrast conventions, as Stage1Trainer), the fragment shader on every covered sample (n2m_s1_asset_shade:
+    nearest texel, specular_net in fp32 with the view direction normalize(x - campos)), optionally dr.antialias, then the evaluation
+    compose of Stage1Trainer.render (n2m_s1_render_compose).  Returns (image [h0*w0,3], weights_sum [h0*w0], depth [h0*w0]).
+    ssaa=1 without antialias is pixel for pixel what the viewer draws; ssaa=2 with antialias compares with Stage1Trainer.render."""
+    from .stage1 import bg_image
+    if shading not in SHADE_MODES:
+        raise ValueError(f"shading must be one of {sorted(SHADE_MODES)}")
+    ssaa = int(ssaa)
+    if ssaa not in (1, 2):
+        raise ValueError("ssaa must be 1 or 2")
+    dev = asset.vertices.device
+    h0, w0 = int(h0), int(w0)
+    h, w = h0 * ssaa, w0 * ssaa
+    Q = h0 * w0
+    bg = bg_image(bg_color, Q, dev)
+    cam = [float(x) for x in (campos.tolist() if torch.is_tensor(campos) else np.asarray(campos, dtype=np.float64).ravel())]
+    mvp = mvp.to(dev, torch.float32).contiguous()
+    vclip = (torch.nn.functional.pad(asset.vertices, (0, 1), value=1.0) @ mvp.T).contiguous()
+    rast, _ = dr.rasterize(glctx or dr.RasterizeCudaContext(dev), vclip[None], asset.triangles, (h, w))
+    img = torch.empty(h * w, 4, device=dev)
+    call("n2m_s1_asset_shade", ptr(rast), h * w, ptr(asset.vertices), ptr(asset.triangles), ptr(asset.st), ptr(asset.ft), ptr(asset._offsets),
+         asset.cascades, ptr(asset._feat0_ptrs), ptr(asset._feat1_ptrs), ptr(asset._tex_size), ptr(asset._mlp), cam[0], cam[1], cam[2],
+         SHADE_MODES[shading], ptr(img), stream())
+    if antialias:
+        th = asset.topology()
+        aa = torch.empty_like(img)
+        call("n2m_antialias_forward", ptr(img), ptr(rast), ptr(vclip), ptr(asset.triangles), ptr(th.keys), ptr(th.opp), th.slots, h, w, 4,
+             ptr(aa), stream())
+        img = aa
+    image = torch.empty(Q, 3, device=dev); weights_sum = torch.empty(Q, device=dev); depth = torch.empty(Q, device=dev)
+    call("n2m_s1_render_compose", ptr(img), ptr(rast), ptr(bg), h0, w0, ssaa, ptr(image), ptr(weights_sum), ptr(depth), stream())
+    return image, weights_sum, depth

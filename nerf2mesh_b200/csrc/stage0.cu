@@ -277,6 +277,15 @@ __device__ __forceinline__ float tv_grad(const TableEntry* __restrict__ tab, con
 // contributions are first summed across each run of same-cell lanes with a segmented warp scan and only the
 // last lane of a run issues the red.global.add.v4.f32.  Fine levels (every lane its own cell) go straight to the atomics.
 //
+// Duplicate rows of neighbouring cells are not summed first.  Adjacent cells share corners, so on bench's lego batch the run merge
+// leaves 69.9 REDs per sample for 48.7 distinct rows per 128-sample tile (per-level counts: profiles/grid_pass_time.py).  But the RED
+// count alone does not bound this kernel: it issues those 19.9 M REDs at 56 G/s, where a kernel that only fires random REDs into one
+// 8 MiB slice reaches 89 G/s.  Measured on an H100 80GB HBM3 (700 W), the scatter of one lego part takes 195 us with the code
+// below.  Summing rows in a 1024-slot open-addressing table in shared memory first -- fp32 CAS loops (there is no shared fp32
+// atomic add) or one 128-bit CAS per contribution, per CTA or per warp, at the levels below a cut from 5 to 13 -- took 266-470 us.
+// Handing the corners shared with the previous issuing lane's cell over by shuffles took 182 us, but 391 us instead of 357 for the
+// whole batch and more on garden (64 registers, 8 CTAs per SM), and left the step's concurrent backward passes no faster.
+//
 // Level-group walk.  The RED target is the whole gradient table: 6.1 M float4 rows = 97.6 MB at the default config (16 levels,
 // 2^19 rows per hashed level), twice the H100's 50 MB L2.  A thread that walks all 16 levels of its sample sends its REDs anywhere
 // in those 97.6 MB, so most of them miss L2 and cost a sector fill plus a write-back.  The work items of a launch are therefore
@@ -753,15 +762,23 @@ static inline uint32_t part_grid(uint32_t Mcap, uint32_t nparts) {
 // them, so the level groups' slices of the gradient table are each filled and written back once per part.  Sharing the device,
 // the parts walk the groups side by side and meet in the same slice.  On an H100 80GB HBM3 (700 W) this took the two lego parts'
 // scatters from 428 to 394 us and the lego step from 1.176 to 1.131 ms.
+// `share`: the launch takes only 1/share of the resident CTAs (see kTvDeviceShare).
 template <bool SCATTER, bool TV>
-static uint32_t encode_bwd_grid(uint32_t Mcap, uint32_t nparts) {
+static uint32_t encode_bwd_grid(uint32_t Mcap, uint32_t nparts, uint32_t share = 1) {
     static int per_sm = 0;
     if (!per_sm) {
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_s0_encode_bwd<SCATTER, TV>, kTile, 0);
         if (per_sm <= 0) per_sm = 1;
     }
-    return min(max(1u, (uint32_t)(per_sm * num_sms()) / nparts), kLevelGroups * part_grid(Mcap, nparts));
+    return min(max(1u, (uint32_t)(per_sm * num_sms()) / (nparts * share)), kLevelGroups * part_grid(Mcap, nparts));
 }
+
+// The TV launch gets half of the device.  The step forks it at its start, beside the parts' gather -> MLP -> composite chains.  A
+// grid of every CTA the device holds at once is a persistent grid-stride walk that keeps its slots until the last item, so the
+// kernels of those chains find no room on the SMs beside it; with half the slots TV runs underneath them.  On an H100 80GB HBM3
+// (700 W) this took the lego step from 1.139-1.142 to 1.076 ms and the garden step from 2.463-2.472 to 2.328-2.331 ms.  A third
+// of the device measured 1.083 / 2.327 ms, a quarter 1.081 / 2.363 ms, a sixth 1.121 ms on lego.
+constexpr uint32_t kTvDeviceShare = 2;
 
 extern "C" {
 
@@ -894,7 +911,7 @@ int n2m_s0_tv(const n2m_s0_params* p, const void* recs, const int32_t* counters,
     N2M_REQUIRE(p && recs && counters && rays_o && rays_d && table && offsets && gtable && loss_scale, "s0_tv", "null pointer");
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_tv", "Mcap must be a positive multiple of 128");
     if (!(p->lambda_tv > 0)) return 0;
-    k_s0_encode_bwd<false, true><<<encode_bwd_grid<false, true>(Mcap, 1), kTile, 0, as_stream(stream)>>>(
+    k_s0_encode_bwd<false, true><<<encode_bwd_grid<false, true>(Mcap, 1, kTvDeviceShare), kTile, 0, as_stream(stream)>>>(
         *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, nullptr, static_cast<const TableEntry*>(table), offsets,
         static_cast<float4*>(gtable), const_cast<float*>(loss_scale), 0, 1);
     return check_launch("s0_tv");

@@ -11,6 +11,9 @@ gradients), then times with CUDA events over many warm launches
 The bytes each pass must move are computed from the shapes: the streamed per-sample data (march records, tile images) plus one pass
 over the 32 B sectors of the tables the batch actually touches (a sector of the gradient table is filled and written back once, a
 sector of the parameter table is read once).  The touched sectors are counted from the gradient table one scatter leaves behind.
+The scatter's RED counts per level ("reds") are computed with torch from the batch's own march records: the 8 corner contributions
+of every sample inside the grid, the REDs the same-cell run merge of a warp leaves, and the distinct gradient rows per 32-sample warp
+and per 128-sample tile (what a scatter that sums duplicate rows per warp / per tile would issue).
 Prints one JSON line per workload with the device name and its power limit.
 """
 import argparse
@@ -34,6 +37,67 @@ def power_limit():
         return r.stdout.strip() or None
     except Exception:      # noqa: BLE001
         return None
+
+
+def red_counts(tr, M):
+    """Per level: corner contributions, REDs left by the warp's same-cell run merge (csrc/stage0.cu encode_bwd_visit), distinct
+    gradient rows per warp and per tile, over the whole batch (positions restated from the records as sample_of / corners_of form
+    them; a sample within an ulp of a cell face may land in the neighbouring cell, which does not matter for a count)."""
+    import numpy as np
+    p, dev = tr.params, tr.recs.device
+    recs = tr.recs[:M]
+    n = recs[:, 3].contiguous().view(torch.int32).long()
+    x = (tr.rays_o[n].double() + recs[:, :1].double() * tr.rays_d[n].double()).float().clamp(-p.bound, p.bound)
+    if p.contract:
+        mag = x.abs().amax(-1, keepdim=True)
+        x = torch.where(mag > 1, x * ((2 - 1 / mag) / mag), x)
+    u = (x + p.grid_bound) * p.inv_2gb
+    T = (M + 127) // 128
+    Mt = T * 128
+    act = torch.zeros(Mt, dtype=torch.bool, device=dev)
+    act[:M] = ((u >= 0) & (u <= 1)).all(-1)
+    u = torch.nn.functional.pad(u, (0, 0, 0, Mt - M), value=0.5)
+    offs = tr._offsets_host
+    out = {"contrib": [], "reds_run_merge": [], "distinct_warp": [], "distinct_tile": []}
+    for l in range(p.num_levels):
+        rows = offs[l + 1] - offs[l]
+        scale = float(np.float32(np.exp2(np.float32(l) * np.float32(p.S)) * np.float32(p.base_res) - np.float32(1)))
+        res = int(np.ceil(scale)) + 1
+        b = torch.floor(u * scale + 0.5).long()
+        s1, stride, mult = res + 1, 1, []
+        for _ in range(3):
+            mult.append(stride if stride <= rows else 0)
+            if stride <= rows:
+                stride *= s1
+        hashed = stride > rows
+        corner = []
+        for k in range(8):
+            c = b + torch.tensor([k & 1, (k >> 1) & 1, (k >> 2) & 1], device=dev)
+            if hashed:
+                raw = (c[:, 0] ^ ((c[:, 1] * 2654435761) & 0xffffffff) ^ ((c[:, 2] * 805459861) & 0xffffffff)) & 0xffffffff
+            else:
+                raw = c[:, 0] * mult[0] + c[:, 1] * mult[1] + c[:, 2] * mult[2]
+            corner.append(raw % rows)
+        corner = torch.stack(corner, 1)
+        key = torch.where(act, b[:, 0] | (b[:, 1] << 10) | (b[:, 2] << 20), torch.full_like(b[:, 0], -1)).view(-1, 32)
+        heads = torch.ones_like(key, dtype=torch.bool)
+        heads[:, 1:] = key[:, 1:] != key[:, :-1]
+        tails = torch.ones_like(heads)
+        tails[:, :-1] = heads[:, 1:]
+        merge = ((heads.sum(1) <= 20) & (res < 1023)).unsqueeze(1)
+        a32 = act.view(-1, 32)
+        issue = torch.where(merge, tails & a32, a32)
+        j = torch.arange(Mt, device=dev).unsqueeze(1).expand(-1, 8)[act]
+        rr = corner[act]
+
+        def distinct(width):
+            return int(torch.unique((j // width) * rows + rr).numel())
+        out["contrib"].append(int(act.sum().item()) * 8)
+        out["reds_run_merge"].append(int(issue.sum().item()) * 8)
+        out["distinct_warp"].append(distinct(32))
+        out["distinct_tile"].append(distinct(128))
+    out["per_sample"] = {k: round(sum(v) / max(M, 1), 2) for k, v in out.items()}
+    return out
 
 
 def run(workload, iters, warmup):
@@ -120,7 +184,7 @@ def run(workload, iters, warmup):
     props = torch.cuda.get_device_properties(0)
     return {"workload": workload, "device": props.name, "power_limit": power_limit(), "M": M, "rows": R,
             "rows_touched": rows_touched, "gtable_sectors_touched": g_sectors, "table_sectors_touched": t_sectors,
-            **res, "iters": iters, "warmup": warmup}
+            **res, "reds": red_counts(tr, M), "iters": iters, "warmup": warmup}
 
 
 def main():

@@ -139,6 +139,29 @@ int n2m_s1_vert_step_world(const float* grad_vclip, const float* grad_vworld, co
                            float lambda_lap, float lambda_offsets, float lr_vert, float eps, const float* opt_state, float* vert_state,
                            float* loss_out, n2m_stream_t stream);
 
+/* mesh regularisers of the vertex offsets (utils.py:759-769: lambda_normal * pytorch3d mesh_normal_consistency + lambda_edgelen *
+ * pytorch3d mesh_edge_loss with target length 0), over the edge hash of n2m_antialias_topology (topo_keys, topo_opp, topo_slots).
+ * n2m_s1_mesh_reg_setup (once per mesh; synchronises `stream`): counts[0] = E, the unique edges (occupied slots), counts[1] = P, the
+ *   edges with exactly two faces, counts[2] = edges with more than two faces (the hash keeps two of them: the normal term needs a mesh
+ *   without), counts[3] = faces with a repeated vertex index; counts is host memory [4], scratch device memory [topo_slots + 4] u32.
+ * n2m_s1_mesh_reg: for vertices [V,3], ACCUMULATES into grad [V,3] the gradient of
+ *   lambda_edgelen / E * sum_edges |v_a - v_b|^2 + lambda_normal / P * sum_pairs (1 - cos(n_c, -n_d))
+ *   with n_c = (v_b - v_a) x (v_c - v_a), n_d likewise, for the edge (a < b) and the opposite vertices c, d of its two faces; cos as
+ *   torch.cosine_similarity(eps = 1e-8) computes and differentiates it (each vector divided by max(|n|, eps)); loss_out (nullable) += the
+ *   value.  A weight whose count (E or P) is 0 contributes nothing.
+ * n2m_s1_vert_step_reg: n2m_s1_vert_step with grad_vworld nullable (non-null: n2m_s1_vert_step_world's image-loss part) and both
+ *   regularisers added to the gradient and to loss_out, on vertices before the update; scratch [9 V] f32.  With lambda_normal =
+ *   lambda_edgelen = 0 it is n2m_s1_vert_step / n2m_s1_vert_step_world. */
+int n2m_s1_mesh_reg_setup(const int32_t* tri, uint32_t F, const void* topo_keys, uint32_t topo_slots, uint32_t* scratch, uint32_t* counts,
+                          n2m_stream_t stream);
+int n2m_s1_mesh_reg(const void* topo_keys, const int32_t* topo_opp, uint32_t topo_slots, uint32_t num_edges, uint32_t num_pairs,
+                    const float* vertices, float lambda_normal, float lambda_edgelen, float* grad, float* loss_out, n2m_stream_t stream);
+int n2m_s1_vert_step_reg(const float* grad_vclip, const float* grad_vworld, const float* mvp, const void* topo_keys, const int32_t* topo_opp,
+                         uint32_t topo_slots, uint32_t num_edges, uint32_t num_pairs, const float* base, float* offsets, float* m, float* v,
+                         float* vertices, float* scratch, float* grad_out, uint32_t V, float lambda_lap, float lambda_offsets, float lambda_normal,
+                         float lambda_edgelen, float lr_vert, float eps, const float* opt_state, float* vert_state, float* loss_out,
+                         n2m_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

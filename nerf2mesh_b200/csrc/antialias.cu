@@ -21,17 +21,11 @@
 // All geometry is evaluated relative to the foreground pixel's centre, so the fp32 decisions (straddle, 0 < t < 1, fold test) agree
 // with the float64 oracle except for crossings within rounding of a pixel centre.
 #include "n2m_common.cuh"
+#include "topology_hash.cuh"
 #include "../../include/n2m_b200_raster.h"
 
 namespace n2m {
 namespace {
-
-constexpr unsigned long long kEmptyKey = ~0ull;
-
-__device__ __forceinline__ uint32_t aa_hash(unsigned long long k) {
-    k ^= k >> 33; k *= 0xff51afd7ed558ccdull; k ^= k >> 33; k *= 0xc4ceb9fe1a85ec53ull; k ^= k >> 33;
-    return (uint32_t)k;
-}
 
 __global__ void __launch_bounds__(256)
 k_aa_topology(const int32_t* __restrict__ tri, uint32_t F, unsigned long long* __restrict__ keys, int32_t* __restrict__ opp, uint32_t mask) {

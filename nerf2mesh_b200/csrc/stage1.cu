@@ -30,6 +30,7 @@
 #include "n2m_common.cuh"
 #include "raster_grad.cuh"
 #include "s0_geom.cuh"
+#include "topology_hash.cuh"
 #include "../../include/n2m_b200_raster.h"
 
 namespace n2m {
@@ -426,13 +427,14 @@ k_s1_vert_check(const float* __restrict__ g, uint32_t n, float* __restrict__ st)
 // grad = (grad_vclip . mvp[:, :3]) / loss_scale + (lambda_lap / V) * (L w) + (2 lambda_offsets / V) * offsets; Adam(eps) on the offsets with
 // its own step count vst[0]; vertices = base + offsets.  Skipped as a whole when found_inf is set (st[3]).  WORLD: the image-loss part is
 // (grad_vclip . mvp[:, :3] + grad_vworld) / loss_scale (the colour-field path, k_s1_offset_grad); grad_vworld is the last parameter, so
-// the WORLD = false instantiation keeps the parameter offsets, and the code, of the kernel without it.
-template <bool WORLD>
-__global__ void __launch_bounds__(256)
-k_s1_vert_adam(const float4* __restrict__ grad_vclip, const float* __restrict__ mvp, const float* __restrict__ lap_grad, const float* __restrict__ base,
-               float* __restrict__ offsets, float* __restrict__ m, float* __restrict__ v, float* __restrict__ vertices, float* __restrict__ grad_out,
-               uint32_t V, float lambda_lap, float lambda_offsets, float lr, float eps, const float* __restrict__ st, const float* __restrict__ vst,
-               const float* __restrict__ grad_vworld) {
+// the WORLD = false instantiation keeps the parameter offsets, and the code, of the kernel without it.  REG (the overload below):
+// reg_grad [V,3] (the mesh regularisers' gradient, k_s1_mesh_reg, already weighted) is added to the gradient and grad_vworld is nullable.
+template <bool WORLD, bool REG>
+__device__ __forceinline__ void vert_adam(const float4* __restrict__ grad_vclip, const float* __restrict__ mvp, const float* __restrict__ lap_grad,
+                                          const float* __restrict__ base, float* __restrict__ offsets, float* __restrict__ m, float* __restrict__ v,
+                                          float* __restrict__ vertices, float* __restrict__ grad_out, uint32_t V, float lambda_lap,
+                                          float lambda_offsets, float lr, float eps, const float* __restrict__ st, const float* __restrict__ vst,
+                                          const float* __restrict__ grad_vworld, const float* __restrict__ reg_grad) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= V) return;
     if (lr < 0.f) lr = vst[1];                                          // learning rate kept on the device (graph-replayed steps)
@@ -446,9 +448,11 @@ k_s1_vert_adam(const float4* __restrict__ grad_vclip, const float* __restrict__ 
         const size_t j = 3 * (size_t)i + c;
         float gi;
         if constexpr (WORLD) gi = (gc.x * mvp[c] + gc.y * mvp[4 + c] + gc.z * mvp[8 + c] + gc.w * mvp[12 + c] + grad_vworld[j]) * inv_scale;
+        else if constexpr (REG) gi = (gc.x * mvp[c] + gc.y * mvp[4 + c] + gc.z * mvp[8 + c] + gc.w * mvp[12 + c] + (grad_vworld ? grad_vworld[j] : 0.f)) * inv_scale;
         else gi = (gc.x * mvp[c] + gc.y * mvp[4 + c] + gc.z * mvp[8 + c] + gc.w * mvp[12 + c]) * inv_scale;
         const float off = offsets[j];
-        const float g = gi + (lambda_lap > 0.f ? lambda_lap / (float)V * lap_grad[j] : 0.f) + 2.f * lambda_offsets / (float)V * off;
+        float g = gi + (lambda_lap > 0.f ? lambda_lap / (float)V * lap_grad[j] : 0.f) + 2.f * lambda_offsets / (float)V * off;
+        if constexpr (REG) g += reg_grad[j];
         if (grad_out) grad_out[j] = g;
         if (skip) continue;
         const float mi = 0.9f * m[j] + 0.1f * g;
@@ -459,6 +463,151 @@ k_s1_vert_adam(const float4* __restrict__ grad_vclip, const float* __restrict__ 
         offsets[j] = o2;
         vertices[j] = base[j] + o2;
     }
+}
+
+template <bool WORLD>
+__global__ void __launch_bounds__(256)
+k_s1_vert_adam(const float4* __restrict__ grad_vclip, const float* __restrict__ mvp, const float* __restrict__ lap_grad, const float* __restrict__ base,
+               float* __restrict__ offsets, float* __restrict__ m, float* __restrict__ v, float* __restrict__ vertices, float* __restrict__ grad_out,
+               uint32_t V, float lambda_lap, float lambda_offsets, float lr, float eps, const float* __restrict__ st, const float* __restrict__ vst,
+               const float* __restrict__ grad_vworld) {
+    vert_adam<WORLD, false>(grad_vclip, mvp, lap_grad, base, offsets, m, v, vertices, grad_out, V, lambda_lap, lambda_offsets, lr, eps, st, vst,
+                            grad_vworld, nullptr);
+}
+
+// the mesh-regulariser step: one overload serves it with and without the colour-field path (grad_vworld nullable)
+__global__ void __launch_bounds__(256)
+k_s1_vert_adam(const float4* __restrict__ grad_vclip, const float* __restrict__ mvp, const float* __restrict__ lap_grad, const float* __restrict__ base,
+               float* __restrict__ offsets, float* __restrict__ m, float* __restrict__ v, float* __restrict__ vertices, float* __restrict__ grad_out,
+               uint32_t V, float lambda_lap, float lambda_offsets, float lr, float eps, const float* __restrict__ st, const float* __restrict__ vst,
+               const float* __restrict__ grad_vworld, const float* __restrict__ reg_grad) {
+    vert_adam<false, true>(grad_vclip, mvp, lap_grad, base, offsets, m, v, vertices, grad_out, V, lambda_lap, lambda_offsets, lr, eps, st, vst,
+                           grad_vworld, reg_grad);
+}
+
+// ---- mesh regularisers of the vertex offsets (utils.py:759-769: lambda_normal * mesh_normal_consistency + lambda_edgelen * mesh_edge_loss of
+// pytorch3d, on vertices = base + offsets before the update), over the slots of the edge hash (csrc/topology_hash.cuh) ----
+// once per mesh: faces per slot into cnt[slot] (one thread per face, one probe per edge with two distinct ends), and faces with a repeated
+// vertex index into res[3]
+__global__ void __launch_bounds__(256)
+k_s1_mesh_reg_faces(const int32_t* __restrict__ tri, uint32_t F, const unsigned long long* __restrict__ keys, uint32_t mask,
+                    uint32_t* __restrict__ cnt, uint32_t* __restrict__ res) {
+    const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
+    if (f >= F) return;
+    const int v[3] = {tri[3 * f], tri[3 * f + 1], tri[3 * f + 2]};
+    if (v[0] == v[1] || v[1] == v[2] || v[0] == v[2]) atomicAdd(res + 3, 1u);
+#pragma unroll
+    for (int e = 0; e < 3; ++e) {
+        const int a = v[e], b = v[(e + 1) % 3];
+        if (a == b) continue;
+        const int64_t s = topo_find(keys, mask, a, b);
+        if (s >= 0) atomicAdd(cnt + s, 1u);
+    }
+}
+
+// res[0] += occupied slots (E, the unique edges), res[1] += slots with exactly two faces (P, the normal pairs), res[2] += slots with more
+__global__ void __launch_bounds__(256)
+k_s1_mesh_reg_slots(const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ cnt, uint32_t slots, uint32_t* __restrict__ res) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool occ = i < slots && keys[i] != kEmptyKey;
+    const uint32_t c = occ ? cnt[i] : 0u;
+    const uint32_t ne = __popc(__ballot_sync(0xffffffffu, occ)), np = __popc(__ballot_sync(0xffffffffu, c == 2u)),
+                   nm = __popc(__ballot_sync(0xffffffffu, c > 2u));
+    if ((threadIdx.x & 31) == 0) {
+        if (ne) atomicAdd(res, ne);
+        if (np) atomicAdd(res + 1, np);
+        if (nm) atomicAdd(res + 2, nm);
+    }
+}
+
+constexpr float kCosEps = 1e-8f;          // torch.cosine_similarity's default eps (mesh_normal_consistency uses the default)
+
+__device__ __forceinline__ void cross3(const float a[3], const float b[3], float r[3]) {
+    r[0] = a[1] * b[2] - a[2] * b[1]; r[1] = a[2] * b[0] - a[0] * b[2]; r[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// One thread per slot; the slot holds edge (a, b), a < b, and the opposite vertices c, d of up to two faces.
+//   edge:   we * |v_a - v_b|^2,  we = lambda_edgelen / E
+//   normal (two faces): wn * (1 - cos(n_c, -n_d)),  wn = lambda_normal / P,  n_c = (v_b - v_a) x (v_c - v_a), n_d likewise; torch's
+//           cosine_similarity divides each vector by max(|n|, eps) and differentiates the branch taken, so a zero-area face gives 1 - 0 and
+//           the gradient n_other / eps.  With both norms >= eps, 1 - cos = |u + w|^2 / 2 for the unit vectors u = n_c / |n_c|,
+//           w = n_d / |n_d|, and d/dn_c = (u + w - loss u) / |n_c|: no cancellation between nearly opposite unit vectors on a smooth mesh.
+// The gradient w.r.t. the vertices is ACCUMULATED into grad [V,3] (6 atomics per edge, 12 per edge with a pair); loss_out[0] += the sum.
+__global__ void __launch_bounds__(256)
+k_s1_mesh_reg(const unsigned long long* __restrict__ keys, const int32_t* __restrict__ opp, uint32_t slots, const float* __restrict__ x,
+              float wn, float we, float* __restrict__ grad, float* __restrict__ loss_out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    float loss = 0.f;
+    const unsigned long long k = i < slots ? keys[i] : kEmptyKey;
+    if (k != kEmptyKey) {
+        const uint32_t a = (uint32_t)(k >> 32), b = (uint32_t)(k & 0xffffffffull);
+        float pa[3], e[3], ga[3], gb[3];
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            pa[c] = x[3 * (size_t)a + c];
+            e[c] = x[3 * (size_t)b + c] - pa[c];
+            ga[c] = 0.f; gb[c] = 0.f;
+        }
+        if (we > 0.f) {
+            loss += we * (e[0] * e[0] + e[1] * e[1] + e[2] * e[2]);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) { ga[c] = -2.f * we * e[c]; gb[c] = 2.f * we * e[c]; }
+        }
+        const int oc = opp[2 * (size_t)i], od = opp[2 * (size_t)i + 1];
+        if (wn > 0.f && od >= 0) {
+            float qc[3], qd[3], nc[3], nd[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) { qc[c] = x[3 * (size_t)oc + c] - pa[c]; qd[c] = x[3 * (size_t)od + c] - pa[c]; }
+            cross3(e, qc, nc);
+            cross3(e, qd, nd);
+            const float lc = __fsqrt_rn(nc[0] * nc[0] + nc[1] * nc[1] + nc[2] * nc[2]);
+            const float ld = __fsqrt_rn(nd[0] * nd[0] + nd[1] * nd[1] + nd[2] * nd[2]);
+            const float rc = __frcp_rn(fmaxf(lc, kCosEps)), rd = __frcp_rn(fmaxf(ld, kCosEps));
+            float u[3], w[3], gc[3], gd[3];
+#pragma unroll
+            for (int c = 0; c < 3; ++c) { u[c] = nc[c] * rc; w[c] = nd[c] * rd; }
+            float L;
+            if (lc >= kCosEps && ld >= kCosEps) {
+                float s[3];
+#pragma unroll
+                for (int c = 0; c < 3; ++c) s[c] = u[c] + w[c];
+                L = 0.5f * (s[0] * s[0] + s[1] * s[1] + s[2] * s[2]);
+#pragma unroll
+                for (int c = 0; c < 3; ++c) { gc[c] = (s[c] - L * u[c]) * rc; gd[c] = (s[c] - L * w[c]) * rd; }
+            } else {
+                const float dp = u[0] * w[0] + u[1] * w[1] + u[2] * w[2];
+                L = 1.f + dp;
+                const float pc = lc >= kCosEps ? dp : 0.f, pd = ld >= kCosEps ? dp : 0.f;        // the clamped branch has no projection
+#pragma unroll
+                for (int c = 0; c < 3; ++c) { gc[c] = (w[c] - pc * u[c]) * rc; gd[c] = (u[c] - pd * w[c]) * rd; }
+            }
+            loss += wn * L;
+#pragma unroll
+            for (int c = 0; c < 3; ++c) { gc[c] *= wn; gd[c] *= wn; }
+            // n = e x q: d/de = q x g, d/dq = g x e; e = v_b - v_a, q = v_o - v_a
+            float t1[3], t2[3], gqc[3], gqd[3];
+            cross3(qc, gc, t1);
+            cross3(qd, gd, t2);
+            cross3(gc, e, gqc);
+            cross3(gd, e, gqd);
+#pragma unroll
+            for (int c = 0; c < 3; ++c) {
+                const float ge = t1[c] + t2[c];
+                gb[c] += ge;
+                ga[c] -= ge + gqc[c] + gqd[c];
+                atomicAdd(grad + 3 * (size_t)oc + c, gqc[c]);
+                atomicAdd(grad + 3 * (size_t)od + c, gqd[c]);
+            }
+        }
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+            atomicAdd(grad + 3 * (size_t)a + c, ga[c]);
+            atomicAdd(grad + 3 * (size_t)b + c, gb[c]);
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) loss += __shfl_xor_sync(0xffffffffu, loss, o);
+    if (loss_out && (threadIdx.x & 31) == 0 && loss != 0.f) atomicAdd(loss_out, loss);
 }
 
 __global__ void k_s1_vert_tick(const float* __restrict__ st, float* __restrict__ vst) {
@@ -594,16 +743,52 @@ int n2m_s1_offset_grad(const n2m_s0_params* p, const float* rast, const float* v
     return check_launch("s1_offset_grad");
 }
 
-static int s1_vert_step(const float* grad_vclip, const float* grad_vworld, const float* mvp, const void* topo_keys, uint32_t topo_slots,
-                        const float* base, float* offsets, float* m, float* v, float* vertices, float* scratch, float* grad_out, uint32_t V,
-                        float lambda_lap, float lambda_offsets, float lr_vert, float eps, const float* opt_state, float* vert_state, float* loss_out,
+int n2m_s1_mesh_reg_setup(const int32_t* tri, uint32_t F, const void* topo_keys, uint32_t topo_slots, uint32_t* scratch, uint32_t* counts,
+                          n2m_stream_t stream) {
+    N2M_REQUIRE(tri && topo_keys && scratch && counts, "s1_mesh_reg_setup", "null pointer");
+    N2M_REQUIRE(topo_slots && !(topo_slots & (topo_slots - 1)), "s1_mesh_reg_setup", "slots must be a power of two");
+    cudaStream_t st = as_stream(stream);
+    const unsigned long long* keys = static_cast<const unsigned long long*>(topo_keys);
+    uint32_t* res = scratch + topo_slots;
+    cudaError_t e = cudaMemsetAsync(scratch, 0, ((size_t)topo_slots + 4) * sizeof(uint32_t), st);
+    if (e != cudaSuccess) return fail("s1_mesh_reg_setup(memset)", cudaGetErrorString(e));
+    if (F > 0) {
+        k_s1_mesh_reg_faces<<<div_up(F, 256u), 256, 0, st>>>(tri, F, keys, topo_slots - 1, scratch, res);
+        if (int err = check_launch("s1_mesh_reg_setup(faces)")) return err;
+    }
+    k_s1_mesh_reg_slots<<<div_up(topo_slots, 256u), 256, 0, st>>>(keys, scratch, topo_slots, res);
+    if (int err = check_launch("s1_mesh_reg_setup(slots)")) return err;
+    e = cudaMemcpyAsync(counts, res, 4 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) return fail("s1_mesh_reg_setup(read)", cudaGetErrorString(e));
+    return 0;
+}
+
+int n2m_s1_mesh_reg(const void* topo_keys, const int32_t* topo_opp, uint32_t topo_slots, uint32_t num_edges, uint32_t num_pairs,
+                    const float* vertices, float lambda_normal, float lambda_edgelen, float* grad, float* loss_out, n2m_stream_t stream) {
+    N2M_REQUIRE(topo_keys && topo_opp && vertices && grad, "s1_mesh_reg", "null pointer");
+    N2M_REQUIRE(lambda_normal >= 0.f && lambda_edgelen >= 0.f, "s1_mesh_reg", "the weights must be >= 0");
+    const float wn = num_pairs ? lambda_normal / (float)num_pairs : 0.f, we = num_edges ? lambda_edgelen / (float)num_edges : 0.f;
+    if (topo_slots == 0 || (wn == 0.f && we == 0.f)) return 0;
+    k_s1_mesh_reg<<<div_up(topo_slots, 256u), 256, 0, as_stream(stream)>>>(static_cast<const unsigned long long*>(topo_keys), topo_opp, topo_slots,
+                                                                          vertices, wn, we, grad, loss_out);
+    return check_launch("s1_mesh_reg");
+}
+
+static int s1_vert_step(const float* grad_vclip, const float* grad_vworld, const float* mvp, const void* topo_keys, const int32_t* topo_opp,
+                        uint32_t topo_slots, uint32_t num_edges, uint32_t num_pairs, const float* base, float* offsets, float* m, float* v,
+                        float* vertices, float* scratch, float* grad_out, uint32_t V, float lambda_lap, float lambda_offsets, float lambda_normal,
+                        float lambda_edgelen, float lr_vert, float eps, const float* opt_state, float* vert_state, float* loss_out,
                         n2m_stream_t stream) {
     N2M_REQUIRE(grad_vclip && mvp && base && offsets && m && v && vertices && scratch && opt_state && vert_state, "s1_vert_step", "null pointer");
     N2M_REQUIRE(lambda_lap <= 0.f || (topo_keys && topo_slots > 0), "s1_vert_step", "the Laplacian term needs the mesh's edge hash");
+    const bool reg = lambda_normal > 0.f || lambda_edgelen > 0.f;
+    N2M_REQUIRE(!reg || (topo_keys && topo_opp && topo_slots > 0), "s1_vert_step", "the mesh regularisers need the mesh's edge hash");
     if (V == 0) return 0;
     cudaStream_t st = as_stream(stream);
     float* u = scratch;                       // [V,3]: L v, then its row-normalised form
     float* lg = scratch + 3 * (size_t)V;      // [V,3]: L (u / |u|)
+    float* rg = scratch + 6 * (size_t)V;      // [V,3]: the mesh regularisers' gradient (reg only)
     if (lambda_lap > 0.f) {
         const unsigned long long* keys = static_cast<const unsigned long long*>(topo_keys);
         cudaError_t e = cudaMemsetAsync(scratch, 0, 6 * (size_t)V * sizeof(float), st);
@@ -615,9 +800,19 @@ static int s1_vert_step(const float* grad_vclip, const float* grad_vworld, const
         k_s1_laplacian<<<div_up(topo_slots, 256u), 256, 0, st>>>(keys, topo_slots, u, lg);
         if (int err = check_launch("s1_vert_step(L w)")) return err;
     }
-    auto adam = grad_vworld ? k_s1_vert_adam<true> : k_s1_vert_adam<false>;
-    adam<<<div_up(V, 256u), 256, 0, st>>>(reinterpret_cast<const float4*>(grad_vclip), mvp, lg, base, offsets, m, v, vertices, grad_out, V,
-                                          lambda_lap, lambda_offsets, lr_vert, eps, opt_state, vert_state, grad_vworld);
+    if (reg) {
+        cudaError_t e = cudaMemsetAsync(rg, 0, 3 * (size_t)V * sizeof(float), st);
+        if (e != cudaSuccess) return fail("s1_vert_step(memset)", cudaGetErrorString(e));
+        if (int err = n2m_s1_mesh_reg(topo_keys, topo_opp, topo_slots, num_edges, num_pairs, vertices, lambda_normal, lambda_edgelen, rg, loss_out,
+                                      stream))
+            return err;
+        k_s1_vert_adam<<<div_up(V, 256u), 256, 0, st>>>(reinterpret_cast<const float4*>(grad_vclip), mvp, lg, base, offsets, m, v, vertices, grad_out,
+                                                        V, lambda_lap, lambda_offsets, lr_vert, eps, opt_state, vert_state, grad_vworld, rg);
+    } else {
+        auto adam = grad_vworld ? k_s1_vert_adam<true> : k_s1_vert_adam<false>;
+        adam<<<div_up(V, 256u), 256, 0, st>>>(reinterpret_cast<const float4*>(grad_vclip), mvp, lg, base, offsets, m, v, vertices, grad_out, V,
+                                              lambda_lap, lambda_offsets, lr_vert, eps, opt_state, vert_state, grad_vworld);
+    }
     if (int err = check_launch("s1_vert_step(adam)")) return err;
     k_s1_vert_tick<<<1, 32, 0, st>>>(opt_state, vert_state);
     return check_launch("s1_vert_step(tick)");
@@ -626,8 +821,19 @@ static int s1_vert_step(const float* grad_vclip, const float* grad_vworld, const
 int n2m_s1_vert_step(const float* grad_vclip, const float* mvp, const void* topo_keys, uint32_t topo_slots, const float* base, float* offsets,
                      float* m, float* v, float* vertices, float* scratch, float* grad_out, uint32_t V, float lambda_lap, float lambda_offsets,
                      float lr_vert, float eps, const float* opt_state, float* vert_state, float* loss_out, n2m_stream_t stream) {
-    return s1_vert_step(grad_vclip, nullptr, mvp, topo_keys, topo_slots, base, offsets, m, v, vertices, scratch, grad_out, V, lambda_lap,
-                        lambda_offsets, lr_vert, eps, opt_state, vert_state, loss_out, stream);
+    return s1_vert_step(grad_vclip, nullptr, mvp, topo_keys, nullptr, topo_slots, 0, 0, base, offsets, m, v, vertices, scratch, grad_out, V,
+                        lambda_lap, lambda_offsets, 0.f, 0.f, lr_vert, eps, opt_state, vert_state, loss_out, stream);
+}
+
+int n2m_s1_vert_step_reg(const float* grad_vclip, const float* grad_vworld, const float* mvp, const void* topo_keys, const int32_t* topo_opp,
+                         uint32_t topo_slots, uint32_t num_edges, uint32_t num_pairs, const float* base, float* offsets, float* m, float* v,
+                         float* vertices, float* scratch, float* grad_out, uint32_t V, float lambda_lap, float lambda_offsets, float lambda_normal,
+                         float lambda_edgelen, float lr_vert, float eps, const float* opt_state, float* vert_state, float* loss_out,
+                         n2m_stream_t stream) {
+    N2M_REQUIRE(lambda_normal >= 0.f && lambda_edgelen >= 0.f, "s1_vert_step_reg", "the weights must be >= 0");
+    return s1_vert_step(grad_vclip, grad_vworld, mvp, topo_keys, topo_opp, topo_slots, num_edges, num_pairs, base, offsets, m, v, vertices, scratch,
+                        grad_out, V, lambda_lap, lambda_offsets, lambda_normal, lambda_edgelen, lr_vert, eps, opt_state, vert_state, loss_out,
+                        stream);
 }
 
 int n2m_s1_vert_step_world(const float* grad_vclip, const float* grad_vworld, const float* mvp, const void* topo_keys, uint32_t topo_slots,
@@ -635,8 +841,8 @@ int n2m_s1_vert_step_world(const float* grad_vclip, const float* grad_vworld, co
                            float lambda_lap, float lambda_offsets, float lr_vert, float eps, const float* opt_state, float* vert_state,
                            float* loss_out, n2m_stream_t stream) {
     N2M_REQUIRE(grad_vworld, "s1_vert_step_world", "null pointer");
-    return s1_vert_step(grad_vclip, grad_vworld, mvp, topo_keys, topo_slots, base, offsets, m, v, vertices, scratch, grad_out, V, lambda_lap,
-                        lambda_offsets, lr_vert, eps, opt_state, vert_state, loss_out, stream);
+    return s1_vert_step(grad_vclip, grad_vworld, mvp, topo_keys, nullptr, topo_slots, 0, 0, base, offsets, m, v, vertices, scratch, grad_out, V,
+                        lambda_lap, lambda_offsets, 0.f, 0.f, lr_vert, eps, opt_state, vert_state, loss_out, stream);
 }
 
 }  // extern "C"

@@ -27,8 +27,12 @@ runs on the concatenated mesh, and `cascade_mesh(cas)` returns one cascade for t
 (renderer.py:223-225) and `replace_mesh` replaces cascade 0, rebasing the outer cascades on their current vertices (:258-285).  With
 Stage0Config(contract=True) the surface points are contracted before the colour field is queried (n2m_s1_points_contract).
 `render()` is render_stage1 at inference (eval_step / test_step, utils.py:853,882): the forward part of the step on buffers of its own, then
-n2m_s1_render_compose -> image, weights_sum, depth, in shading 'diffuse', 'specular' or 'full'.  Not built: the
-pytorch3d regularisers that are off by default (lambda_normal, lambda_edgelen) and SDF mode's all-ones refinement mask.
+n2m_s1_render_compose -> image, weights_sum, depth, in shading 'diffuse', 'specular' or 'full'.
+`lambda_normal` / `lambda_edgelen` (need lr_vert > 0) add the reference's two pytorch3d regularisers of the vertex-offset group
+(utils.py:759-769): lambda_normal * mesh_normal_consistency + lambda_edgelen * mesh_edge_loss over the concatenated mesh of all cascades,
+one walk over the edge hash per step (n2m_s1_vert_step_reg).  The normal term needs a mesh without non-manifold edges (the reference
+repairs them before stage 1 and after every re-mesh, meshutils.py:172-175,211-214), and both need faces of three distinct vertices: such
+meshes raise ValueError at construction and in replace_mesh.  Not built: SDF mode's all-ones refinement mask.
 """
 import ctypes
 
@@ -54,6 +58,9 @@ _lib.register({
     "n2m_s1_offset_grad": [P, P, P, P, P, P, U, U, P, P, P, P, P, P, P, P],
     "n2m_s1_vert_step_world": [P, P, P, P, U, P, P, P, P, P, P, P, U, F, F, F, F, P, P, P, P],
     "n2m_s1_render_compose": [P, P, P, U, U, U, P, P, P, P],
+    "n2m_s1_mesh_reg_setup": [P, U, P, U, P, P, P],
+    "n2m_s1_mesh_reg": [P, P, U, U, U, P, F, F, P, P, P],
+    "n2m_s1_vert_step_reg": [P, P, P, P, P, U, U, U, P, P, P, P, P, P, P, U, F, F, F, F, F, F, P, P, P, P],
 })
 
 # shading -> n2m_s0_params.shading_full of the forward MLP launch ('specular': the specular term alone, evaluation only)
@@ -74,7 +81,7 @@ class Stage1Trainer:
     v_cumsum = f_cumsum = ()            # per-cascade vertex / face offsets, set by _set_cascades
 
     def __init__(self, t0, vertices, triangles, h0, w0, ssaa=2, max_points=None, lambda_mask=0.1, antialias=False, pos_gradient_boost=1.0,
-                 lr_vert=0.0, lambda_lap=0.001, lambda_offsets=0.1, refine=False, offset_nerf_grad=False):
+                 lr_vert=0.0, lambda_lap=0.001, lambda_offsets=0.1, refine=False, offset_nerf_grad=False, lambda_normal=0.0, lambda_edgelen=0.0):
         assert ssaa in (1, 2), "the ssaa average equals the reference's bilinear down-scale only at factors 1 and 2"
         self.t0 = t0
         dev = t0.device
@@ -116,6 +123,13 @@ class Stage1Trainer:
         self.offset_nerf_grad = bool(offset_nerf_grad)
         if self.offset_nerf_grad and not self.lr_vert > 0:
             raise ValueError("offset_nerf_grad trains the vertex offsets: it needs lr_vert > 0 (and with it antialias=True)")
+        # mesh regularisers of the vertex offsets (main.py:86-87, off by default; the reference's recipes use lambda_normal 1e-3 .. 1e-1)
+        self.lambda_normal, self.lambda_edgelen = float(lambda_normal), float(lambda_edgelen)
+        if not (self.lambda_normal >= 0 and self.lambda_edgelen >= 0):
+            raise ValueError("lambda_normal and lambda_edgelen must be >= 0")
+        self.mesh_reg = self.lambda_normal > 0 or self.lambda_edgelen > 0
+        if self.mesh_reg and not self.lr_vert > 0:
+            raise ValueError("lambda_normal / lambda_edgelen regularise the vertex offsets: they need lr_vert > 0 (and with it antialias=True)")
         self.refine = bool(refine)
         self._mesh_buffers()
         # the specular regulariser and TV are stage-0 losses (utils.py:726,735-738)
@@ -148,23 +162,40 @@ class Stage1Trainer:
 
     def _mesh_buffers(self):
         """(re)allocate everything sized by the mesh, for self.vertices / self.triangles: the edge hash, the clip-space vertex gradient,
-        the vertex-offset group (base = vertices, zero offsets and moments) and the per-face error accumulators"""
+        the vertex-offset group (base = vertices, zero offsets and moments), the mesh regularisers' edge / pair counts and the per-face
+        error accumulators"""
         dev = self.t0.device
         V, Fn = self.vertices.shape[0], self.triangles.shape[0]
         if self.antialias:
             self.topology = dr.TopologyHash(self.triangles)               # once per mesh
             self.grad_vclip = torch.zeros(V, 4, device=dev)
+        if self.mesh_reg:
+            # E (unique edges) and P (edges with two faces): the means' denominators, launch constants of every step on this mesh
+            self.mesh_edges, self.mesh_pairs = self._check_mesh_reg(self.topology, "Stage1Trainer")
         if self.lr_vert > 0:
             self.base_vertices = self.vertices.clone()
             self.offsets = torch.zeros(V, 3, device=dev)
             self.m_vert = torch.zeros(V, 3, device=dev); self.v_vert = torch.zeros(V, 3, device=dev)
-            self.vert_scratch = torch.zeros(6 * V, device=dev)
+            # [6V] the Laplacian's two [V,3] vectors, + [3V] the mesh regularisers' gradient
+            self.vert_scratch = torch.zeros((9 if self.mesh_reg else 6) * V, device=dev)
             self.grad_offsets = torch.zeros(V, 3, device=dev)             # total gradient of the last step (diagnostic / tests)
         if self.offset_nerf_grad:
             self.grad_vworld = torch.zeros(V, 3, device=dev)              # colour-field path, world space, loss-scaled
         if self.refine:
             # triangles_errors / triangles_errors_cnt (renderer.py:163-164): summed per-pixel loss and pixel count per face
             self.face_errors = torch.zeros(Fn, device=dev); self.face_counts = torch.zeros(Fn, device=dev)
+
+    def _check_mesh_reg(self, th, where):
+        """(E, P) of the mesh of edge hash `th` for the mesh regularisers; ValueError for faces with a repeated vertex index (pytorch3d
+        would pair such a face with itself) and, with lambda_normal > 0, for edges of three or more faces (the hash keeps two)"""
+        E, P, nonmanifold, repeated = mesh_reg_counts(th)
+        if repeated:
+            raise ValueError(f"{where}: {repeated} faces with a repeated vertex index: lambda_normal / lambda_edgelen need faces of three "
+                             "distinct vertices")
+        if self.lambda_normal > 0 and nonmanifold:
+            raise ValueError(f"{where}: {nonmanifold} non-manifold edges (three or more faces): lambda_normal needs a mesh without; repair "
+                             "them first, as the reference does before stage 1 and after every re-mesh")
+        return E, P
 
     def _pp(self):
         return ctypes.byref(self.params)
@@ -271,6 +302,13 @@ class Stage1Trainer:
         th = self.topology
         if self.lambda_offsets > 0:
             self.loss_acc[0:1].add_(self.lambda_offsets * (self.offsets * self.offsets).sum(1).mean())          # utils.py:764-776
+        if self.mesh_reg:               # + lambda_normal * mesh_normal_consistency + lambda_edgelen * mesh_edge_loss (utils.py:759-769)
+            call("n2m_s1_vert_step_reg", ptr(self.grad_vclip), ptr(self.grad_vworld) if self.offset_nerf_grad else None, ptr(self.mvp),
+                 ptr(th.keys), ptr(th.opp), th.slots, self.mesh_edges, self.mesh_pairs, ptr(self.base_vertices), ptr(self.offsets),
+                 ptr(self.m_vert), ptr(self.v_vert), ptr(self.vertices), ptr(self.vert_scratch), ptr(self.grad_offsets), V, self.lambda_lap,
+                 self.lambda_offsets, self.lambda_normal, self.lambda_edgelen, -1.0, self.t0.cfg.eps, ptr(self.t0.opt_state),
+                 ptr(self.vert_state), ptr(self.loss_acc), stream())
+            return
         rest = (ptr(self.mvp), ptr(th.keys), th.slots, ptr(self.base_vertices), ptr(self.offsets), ptr(self.m_vert), ptr(self.v_vert),
                 ptr(self.vertices), ptr(self.vert_scratch), ptr(self.grad_offsets), V, self.lambda_lap, self.lambda_offsets, -1.0,
                 self.t0.cfg.eps, ptr(self.t0.opt_state), ptr(self.vert_state), ptr(self.loss_acc), stream())
@@ -411,6 +449,8 @@ class Stage1Trainer:
             raise ValueError(f"replace_mesh: triangles index outside the vertices (0..{V - 1})")
         if not bool(torch.isfinite(vertices).all()):
             raise ValueError("replace_mesh: vertices must be finite")
+        if self.mesh_reg:               # checked before anything changes; the outer cascades passed already and no face links two cascades
+            self._check_mesh_reg(dr.TopologyHash(triangles.to(self.t0.device, torch.int32)), "replace_mesh")
         outer = [self.cascade_mesh(cas) for cas in range(1, self.cascades)]
         self._graphs.clear()
         self._warm = False
@@ -427,6 +467,15 @@ class Stage1Trainer:
 
 
 _INT_DTYPES = (torch.int8, torch.uint8, torch.int16, torch.int32, torch.int64)
+
+
+def mesh_reg_counts(th):
+    """(E unique edges, P edges with exactly two faces, edges with more than two faces, faces with a repeated vertex index) of the mesh
+    th.tri over its edge hash `th` (dr.TopologyHash): n2m_s1_mesh_reg_setup, which reads the four counts back to the host"""
+    scratch = torch.empty(th.slots + 4, dtype=torch.int32, device=th.tri.device)
+    counts = (ctypes.c_uint32 * 4)()
+    call("n2m_s1_mesh_reg_setup", ptr(th.tri), th.tri.shape[0], ptr(th.keys), th.slots, ptr(scratch), counts, stream())
+    return tuple(int(c) for c in counts)
 
 
 def _cascade_lists(vertices, triangles):

@@ -78,6 +78,11 @@ int n2m_s0_init(void);
 /* test hook: 1 = sequential one-thread-per-ray marcher, 0 = warp-per-ray marcher (default); same results */
 int n2m_s0_set_serial_march(int on);
 
+/* test hook: launch form of the scatter (n2m_s0_encode_bwd).  0 = chosen from the part count (default), 1 = 128-thread CTAs on the
+ * resident slots of every SM, 2 = 1024-thread CTAs, one per SM, on 1/nparts of the SMs; same results up to the order of the fp32
+ * additions */
+int n2m_s0_set_scatter_form(int form);
+
 /* the TV gradient of the step's samples: reads recs/table, adds into gtable, counts counters[3] / [15]; independent of the MLP kernels,
  * so a host may run it on a forked stream beside them */
 int n2m_s0_tv(const n2m_s0_params* p, const void* recs, const int32_t* counters, uint32_t Mcap, const float* rays_o,

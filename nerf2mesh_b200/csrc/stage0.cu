@@ -324,7 +324,7 @@ encode_bwd_visit(const n2m_s0_params& p, const float4* __restrict__ recs,
                  const int32_t* __restrict__ offsets, float4* __restrict__ gtable, float* __restrict__ loss_scale,
                  const PartRange pr, uint32_t tile, uint32_t l0, uint32_t l1, int32_t* tv_counts) {
     static_assert(SCATTER != TV, "a launch either scatters the feature gradients or evaluates TV");
-    const uint32_t r = threadIdx.x;
+    const uint32_t r = threadIdx.x & (kTile - 1);          // this thread's row of the tile (a CTA may hold several walkers)
     const uint32_t lane = r & 31;
     const uint32_t j = tile * kTile + r;
     Sample s;
@@ -431,6 +431,31 @@ k_s0_encode_bwd(n2m_s0_params p, const float4* __restrict__ recs, const int32_t*
         const uint32_t grp = item / nt;
         encode_bwd_visit<SCATTER, TV>(p, recs, rays_o, rays_d, denc_tiles, table, offsets, gtable, loss_scale, pr, t0 + item % nt,
                                       group_first_level(grp), group_first_level(grp + 1), const_cast<int32_t*>(counters));
+    }
+}
+
+// The whole-SM form of the scatter (see "Launch geometry" below): a CTA of kWholeSmThreads threads is kWholeSmThreads / kTile independent
+// 128-thread walkers, each visiting one (level group, tile) item at a time as a k_s0_encode_bwd CTA does; walker w of the grid starts at
+// item w and strides by the grid's walker count, so the group-major order is kept.  The walkers share nothing (no CTA barrier).  The
+// register cap (the fewest without a spill; the per-item loop of eight walkers needs 8 more than k_s0_encode_bwd) makes a CTA take
+// more than half the register file, so the hardware places one per SM.  A kernel of its own, so that the per-slot form keeps its
+// 48 registers and 10 CTAs per SM.
+constexpr uint32_t kWholeSmThreads = 1024;
+
+__global__ void __maxnreg__(56)
+k_s0_scatter_walkers(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* __restrict__ counters,
+                     const float* __restrict__ rays_o, const float* __restrict__ rays_d, const uint8_t* __restrict__ denc_tiles,
+                     const int32_t* __restrict__ offsets, float4* __restrict__ gtable, float* __restrict__ loss_scale,
+                     uint32_t part, uint32_t nparts) {
+    const PartRange pr = part_range(counters, part, nparts);
+    if (pr.hi <= pr.lo) return;
+    const uint32_t t0 = pr.lo / kTile, nt = (pr.hi + kTile - 1) / kTile - t0;
+#pragma unroll 1
+    for (uint32_t item = blockIdx.x * (kWholeSmThreads / kTile) + threadIdx.x / kTile; item < kLevelGroups * nt;
+         item += gridDim.x * (kWholeSmThreads / kTile)) {
+        const uint32_t grp = item / nt;
+        encode_bwd_visit<true, false>(p, recs, rays_o, rays_d, denc_tiles, nullptr, offsets, gtable, loss_scale, pr, t0 + item % nt,
+                                      group_first_level(grp), group_first_level(grp + 1), nullptr);
     }
 }
 
@@ -755,14 +780,22 @@ static inline uint32_t part_grid(uint32_t Mcap, uint32_t nparts) {
     return nparts <= 1 ? Mcap / kTile : div_up(Mcap / kTile, nparts) + 1;
 }
 
-// blocks for one scatter / TV launch: the CTAs that are resident on the device at once (read once per process), divided among the
-// `nparts` ray-range parts whose scatters the step runs side by side, so that the group-major item order is also the order in
-// which the items run; never more than the launch has items.
-// With a whole-device grid per part, the first part's CTAs hold every SM slot for their whole walk and the next part queues behind
-// them, so the level groups' slices of the gradient table are each filled and written back once per part.  Sharing the device,
-// the parts walk the groups side by side and meet in the same slice.  On an H100 80GB HBM3 (700 W) this took the two lego parts'
-// scatters from 428 to 394 us and the lego step from 1.176 to 1.131 ms.
-// `share`: the launch takes only 1/share of the resident CTAs (see kTvDeviceShare).
+// Launch geometry of one scatter / TV launch.  Every walk is persistent: its CTAs keep their SM resources until the last item, and
+// the launch takes 1/(nparts * share) of the device, so that the walks the step runs side by side (the parts' scatters, TV) each get
+// their own share and walk the level groups at the same time.
+//  * A scatter with nparts > 1 runs beside the other parts' chains, whose k_mlp_bwd (384 threads x 160 registers, 217 KB of shared
+//    memory) only starts on an SM with no other CTA on it.  It takes the whole-SM form (k_s0_scatter_walkers): one CTA per SM on
+//    S / nparts of the S SMs, so the other SMs are free of it as soon as one part's k_mlp_bwd leaves them.  In the per-slot form the
+//    part-0 scatter's CTAs queued behind part 1's k_mlp_bwd on every SM (33 us on lego, 87 us on garden).  On an H100 80GB HBM3
+//    (700 W) this took the lego step from 1.070-1.077 to 1.034-1.036 ms and the garden step from 2.321-2.332 to 2.199-2.207 ms.  A
+//    whole-SM grid of S CTAs per part measured 1.091-1.093 / 2.271-2.283 ms.
+//  * Every other launch (TV; the scatter with nparts == 1: stage 1, the fused forward, single-part stage 0) takes the per-slot form
+//    (k_s0_encode_bwd) on its share of every SM's resident slots: TV runs underneath the forward chains, whose CTAs are small, and a
+//    lone scatter has nothing beside it.  TV in the whole-SM form on half of the SMs measured 1.026-1.030 / 2.259 ms, on a third
+//    1.032-1.034 / 2.220 ms, against 1.032-1.033 / 2.201-2.202 ms for the per-slot TV (scatters whole-SM in all three).
+// Never more CTAs than the launch has items.
+static int g_scatter_form = 0;        // test hook n2m_s0_set_scatter_form: 0 = by part count, 1 = per-slot, 2 = whole-SM
+
 template <bool SCATTER, bool TV>
 static uint32_t encode_bwd_grid(uint32_t Mcap, uint32_t nparts, uint32_t share = 1) {
     static int per_sm = 0;
@@ -771,6 +804,10 @@ static uint32_t encode_bwd_grid(uint32_t Mcap, uint32_t nparts, uint32_t share =
         if (per_sm <= 0) per_sm = 1;
     }
     return min(max(1u, (uint32_t)(per_sm * num_sms()) / (nparts * share)), kLevelGroups * part_grid(Mcap, nparts));
+}
+
+static uint32_t scatter_walkers_grid(uint32_t Mcap, uint32_t nparts) {
+    return min(max(1u, (uint32_t)num_sms() / nparts), div_up(kLevelGroups * part_grid(Mcap, nparts), kWholeSmThreads / kTile));
 }
 
 // The TV launch gets half of the device.  The step forks it at its start, beside the parts' gather -> MLP -> composite chains.  A
@@ -784,6 +821,12 @@ extern "C" {
 
 /* test hook: 1 = one-thread-per-ray sequential marcher (the reference's structure), 0 = warp-per-ray (default) */
 int n2m_s0_set_serial_march(int on) { g_serial_march = on != 0; return 0; }
+/* test hook: launch form of the scatter, 0 = chosen from its part count (default), 1 = per-slot, 2 = whole-SM */
+int n2m_s0_set_scatter_form(int form) {
+    N2M_REQUIRE(form >= 0 && form <= 2, "s0_set_scatter_form", "form must be 0, 1 or 2");
+    g_scatter_form = form;
+    return 0;
+}
 int n2m_s0_pack_tables(const float* emb_density, const float* emb_color, uint32_t rows, void* table, void* color_master,
                        n2m_stream_t stream) {
     N2M_REQUIRE(emb_density && emb_color && table && color_master, "s0_pack_tables", "null pointer");
@@ -898,9 +941,15 @@ int n2m_s0_encode_bwd(const n2m_s0_params* p, const void* recs, const int32_t* c
     N2M_REQUIRE(p->num_levels == kLevels, "s0_encode_bwd", "fused path supports num_levels == 16");
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_encode_bwd", "Mcap must be a positive multiple of 128");
     N2M_REQUIRE(valid_parts(part, nparts), "s0_encode_bwd", "nparts must be 1, 2, 4 or 8 and part < nparts");
-    k_s0_encode_bwd<true, false><<<encode_bwd_grid<true, false>(Mcap, nparts), kTile, 0, as_stream(stream)>>>(
-        *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, static_cast<const uint8_t*>(denc_tiles),
-        static_cast<const TableEntry*>(table), offsets, static_cast<float4*>(gtable), const_cast<float*>(loss_scale), part, nparts);
+    const bool whole_sm = g_scatter_form ? g_scatter_form == 2 : nparts > 1;
+    if (whole_sm)
+        k_s0_scatter_walkers<<<scatter_walkers_grid(Mcap, nparts), kWholeSmThreads, 0, as_stream(stream)>>>(
+            *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, static_cast<const uint8_t*>(denc_tiles), offsets,
+            static_cast<float4*>(gtable), const_cast<float*>(loss_scale), part, nparts);
+    else
+        k_s0_encode_bwd<true, false><<<encode_bwd_grid<true, false>(Mcap, nparts), kTile, 0, as_stream(stream)>>>(
+            *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, static_cast<const uint8_t*>(denc_tiles),
+            static_cast<const TableEntry*>(table), offsets, static_cast<float4*>(gtable), const_cast<float*>(loss_scale), part, nparts);
     return check_launch("s0_encode_bwd");
 }
 

@@ -36,6 +36,7 @@ PP = ctypes.POINTER(S0Params)
 _lib.register({
     "n2m_s0_init": [],
     "n2m_s0_set_serial_march": [I],
+    "n2m_s0_set_scatter_form": [I],
     "n2m_s0_tv": [PP, P, P, U, P, P, P, P, P, P, P],
     "n2m_s0_tv_random": [PP, P, P, P, P, P, U, P, P],
     "n2m_s0_pack_weights": [P, P, P],

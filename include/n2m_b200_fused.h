@@ -30,14 +30,20 @@
  *              51-53 unit view direction, 54-63 zero.  It is the A operand of every first-layer GEMM and is
  *              staged global->shared with a single bulk async copy.
  *   recs       [Mcap] float4 {t_before, dt, t_after, ray_id (bits)} per sample, ray order.
- *   counters   int32 [16]: [0] M (total samples marched), [1] min(M, Mcap), [2] overflow flag, [3] / [15] samples inside / outside the
+ *   counters   int32 [17]: [0] M (total samples marched), [1] min(M, Mcap), [2] overflow flag, [3] / [15] samples inside / outside the
  *              unit cube (counted by the TV pass, read by n2m_s0_tv_random),
- *              [4..12] sample offset of the first ray of every eighth of the batch (ray N*e/8, e = 0..8; [4] = 0,
+ *              [4..12] sample offset of the first ray of every eighth of the batch (ray n*e/8, e = 0..8; [4] = 0,
  *              [12] = [1]): the boundaries of the ray-range parts (see "Ray-range parts" below).
  *              [13] += 1 for every march whose M exceeded Mcap, [14] = largest M seen (persistent capacity accounting: the rays
  *              that do not fit -- always the last rays of the batch -- are rendered as background and get no gradient, which
  *              the reference never does (it allocates exactly M, raymarching.py:232-238); hosts must watch [13] and grow Mcap).
+ *              [16] n, the active ray count of the batch (adaptive ray count only: written by n2m_s0_march when it is given a
+ *              control block; the batch is the first n of the N rows and n = N otherwise).
  *              Entry points without parts (and nparts == 1) read only [1], so hand-filled 4-entry arrays work there.
+ *   ray_ctl    int32 [4], persistent, adaptive ray count only (the reference's --adaptive_num_rays, nerf/utils.py:795-797):
+ *              [0] ray count n of the next march, in [1, N]; the host sets it to the first step's count.  [1] += 1 for every march
+ *              whose requested count exceeded N and was clamped to it; [2] = largest count requested before that clamp (saturated
+ *              at INT32_MAX); [3] unused.  The host zeroes [1] / [2] when it reads them.
  *   wpack      packed fp16 MLP weights in tensor-core tile layout (n2m_s0_pack_weights).
  */
 #ifndef N2M_B200_FUSED_H
@@ -113,11 +119,15 @@ int n2m_s0_unpack_tables(const void* table, const void* color_master, uint32_t r
 int n2m_s0_unpack_grads(const void* gtable, uint32_t rows, const float* loss_scale,
                         float* g_density, float* g_color, n2m_stream_t stream);
 
-/* march: near/far + count + scan + sample records.  cam_near_far [N,2] nullable (renderer.py:689-691). */
+/* march: near/far + count + scan + sample records.  cam_near_far [N,2] nullable (renderer.py:689-691).
+ * ray_ctl (nullable): adaptive ray count.  NULL marches all N rays.  Given a control block the march takes n = min(ray_ctl[0], N), records
+ * n in counters[16], marches rays [0, n) only (rays >= n get zero samples and their rows are never read, NaN included), cuts the parts at
+ * ray n*e/8, and leaves the next march's count in ray_ctl[0]:  rint(((double)num_points / (double)M) * (double)n), M = counters[0]
+ * (never capped by Mcap), clamped to [1, N].  M == 0 keeps n (the reference would divide by zero there). */
 int n2m_s0_march(const n2m_s0_params* p, const float* rays_o, const float* rays_d, const float* aabb,
                  const float* cam_near_far, const uint8_t* bitfield, const float* noises, uint32_t N,
                  int32_t* rays, int32_t* counters, float* tbuf, void* recs, uint32_t Mcap,
-                 n2m_stream_t stream);
+                 int32_t* ray_ctl, uint32_t num_points, n2m_stream_t stream);
 
 /* the hash-grid gather of the march records into enc_tiles */
 int n2m_s0_encode_fwd(const n2m_s0_params* p, const void* recs, const int32_t* counters, uint32_t Mcap,
@@ -162,13 +172,14 @@ int n2m_s0_mlp_fwd(const n2m_s0_params* p, const void* enc_tiles, const int32_t*
 
 /* per ray: composite, loss, composite backward.  gt [N,4] (rgba) or [N,3]; bg [N,3].
  * dout [Mcap] float4 {dL/dsigma, dL/dr, dL/dg, dL/db} * loss_scale (zero beyond each ray's break).
- * loss_out float[4]: [0] += sum_rays per-ray loss / N (rgb + mask + ray-level entropy), [1] is the MLP forward's sum |spec|^2,
+ * loss_out float[4]: [0] += sum_rays per-ray loss / n (rgb + mask + ray-level entropy), [1] is the MLP forward's sum |spec|^2,
  * [2] += sum of H(weights_k) over the weights the compositor touched, [3] += their count (lambda_entropy > 0 only);
- * image/ws/depth [N] outputs. */
+ * image/ws/depth [N] outputs.  active_rays (nullable, = counters + 16 after a march given a control block): the batch is its first
+ * n = *active_rays rays -- the parts, the loss's 1/n and the outputs cover those, rows >= n are neither read nor written; NULL: n = N. */
 int n2m_s0_composite_loss(const n2m_s0_params* p, const void* out, const void* recs, const int32_t* rays,
                           const int32_t* counters, uint32_t N, uint32_t Mcap, const float* gt, const float* bg,
                           const float* loss_scale, void* dout, float* image, float* weights_sum, float* depth,
-                          float* loss_out, uint32_t part, uint32_t nparts, n2m_stream_t stream);
+                          float* loss_out, const int32_t* active_rays, uint32_t part, uint32_t nparts, n2m_stream_t stream);
 
 /* MLP backward: denc_tiles (same tile layout as enc_tiles, fp16, loss-scaled), g_mlp flat fp32 [7648] += */
 int n2m_s0_mlp_bwd(const n2m_s0_params* p, const void* enc_tiles, const void* dout, const int32_t* counters,
@@ -182,7 +193,7 @@ int n2m_s0_encode_bwd(const n2m_s0_params* p, const void* recs, const int32_t* c
                       n2m_stream_t stream);
 
 /* Ray-range parts.  The five stages above between march and optimizer run on part `part` of `nparts` (1, 2, 4 or 8) contiguous
- * ray ranges of the batch -- part k covers rays [N*k/nparts, N*(k+1)/nparts) and their (contiguous, ray-ordered) samples -- so that
+ * ray ranges of the batch -- part k covers rays [n*k/nparts, n*(k+1)/nparts) of its n rays and their (contiguous, ray-ordered) samples -- so that
  * independent chains  gather -> MLP -> composite -> MLP backward -> scatter  of different parts can be in flight on
  * different streams: the latency-bound tensor-core MLP kernels of one part then share the SMs with the memory-bound
  * gather / scatter kernels of another.  A 128-sample tile that straddles a part boundary is computed by both parts,

@@ -99,8 +99,9 @@ __host__ __device__ __forceinline__ uint32_t compact3(uint32_t x) {
 
 
 // ---- ray-range parts of a batch (fused stage-0 path) ----------------------------------------------
-// The march leaves the sample offsets of rays N*e/8 (e = 0..8) in counters[4..12] (clamped to counters[1]).
-// Part `part` of `nparts` (1, 2, 4 or 8) covers rays [N*e0/8, N*e1/8) with e0 = part*8/nparts, e1 = (part+1)*8/nparts,
+// The march leaves the sample offsets of rays n*e/8 (e = 0..8) in counters[4..12] (clamped to counters[1]); n is the batch's active
+// ray count (counters[16], adaptive ray count) or its N rows.
+// Part `part` of `nparts` (1, 2, 4 or 8) covers rays [n*e0/8, n*e1/8) with e0 = part*8/nparts, e1 = (part+1)*8/nparts,
 // i.e. the contiguous samples [counters[4+e0], counters[4+e1]).  nparts == 1 reads only counters[1] (callers that
 // fill counters by hand, e.g. the explicit-point gather, keep working with a 4-entry array).
 constexpr uint32_t kPartSlots = 8;

@@ -17,12 +17,21 @@ using namespace march;
 // ------------------------------------------------------------------------------------------------
 // march
 // ------------------------------------------------------------------------------------------------
+// Adaptive ray count (--adaptive_num_rays): a batch is the first n rays of the N-row buffers.  The march takes n from the control
+// block's ray_ctl[0] (left there by the previous march's scan), the composite from counters[16]; rays >= n march no sample and are
+// never read.  Without a count n = N.
+__device__ __forceinline__ uint32_t ray_count(const int32_t* __restrict__ count, uint32_t N) {
+    return count ? min((uint32_t)max(*count, 1), N) : N;
+}
+
+template <bool ADAPTIVE>
 __global__ void __launch_bounds__(128)
 k_s0_count(const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ aabb,
            const float* __restrict__ cam_nf, const uint8_t* __restrict__ bits, const float* __restrict__ noises,
-           n2m_s0_params p, uint32_t N, int32_t* __restrict__ rays, float2* __restrict__ tbuf) {
+           n2m_s0_params p, uint32_t N, const int32_t* __restrict__ ray_ctl, int32_t* __restrict__ rays, float2* __restrict__ tbuf) {
     const uint32_t n = blockIdx.x * blockDim.x + threadIdx.x;
     if (n >= N) return;
+    if (ADAPTIVE && n >= ray_count(ray_ctl, N)) { rays[2 * n + 1] = 0; return; }
     const MarchCfg c = make_cfg(p.bound, p.contract != 0, p.dt_gamma, p.max_steps, p.cascades, p.grid_size, bits);
     float near, far;
     near_far_aabb(rays_o + 3 * n, rays_d + 3 * n, aabb, p.min_near, near, far);
@@ -47,13 +56,16 @@ k_s0_count(const float* __restrict__ rays_o, const float* __restrict__ rays_d, c
 // cascade, occupancy bit, voxel-exit time: the expensive part), and then replays the sequential control flow
 // over the precomputed probes with ballots: runs of occupied samples are consumed in one go, an empty probe
 // jumps to the first tau that is not < its exit time.  Same visited set, same (t, dt) per sample, bit for bit.
+template <bool ADAPTIVE>
 __global__ void __launch_bounds__(128)
 k_s0_count_warp(const float* __restrict__ rays_o, const float* __restrict__ rays_d, const float* __restrict__ aabb,
                 const float* __restrict__ cam_nf, const uint8_t* __restrict__ bits, const float* __restrict__ noises,
-                n2m_s0_params p, uint32_t N, int32_t* __restrict__ rays, float2* __restrict__ tbuf) {
+                n2m_s0_params p, uint32_t N, const int32_t* __restrict__ ray_ctl, int32_t* __restrict__ rays,
+                float2* __restrict__ tbuf) {
     const uint32_t n = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const uint32_t lane = threadIdx.x & 31;
     if (n >= N) return;
+    if (ADAPTIVE && n >= ray_count(ray_ctl, N)) { if (lane == 0) rays[2 * n + 1] = 0; return; }
     const MarchCfg c = make_cfg(p.bound, p.contract != 0, p.dt_gamma, p.max_steps, p.cascades, p.grid_size, bits);
     float near, far;
     near_far_aabb(rays_o + 3 * n, rays_d + 3 * n, aabb, p.min_near, near, far);
@@ -140,13 +152,20 @@ k_s0_count_warp(const float* __restrict__ rays_o, const float* __restrict__ rays
 }
 
 // single-block exclusive scan (N is a few thousand rays) -> offsets + counters
+// With a control block (adaptive ray count) it also records this batch's n in counters[16] and leaves the next march's count in
+// ray_ctl[0]: the reference's rule, utils.py:795-797, num_rays = int(round((num_points / M) * num_rays)), in float64 and in that order
+// (rint rounds half to even as round() does), M unclamped by Mcap as the reference never caps it, clamped to [1, N].  Steps clamped at N
+// are counted in ray_ctl[1], the largest count asked for before the clamp is kept in ray_ctl[2].  A batch with M == 0 keeps n, where the
+// reference would divide by zero.
 __global__ void __launch_bounds__(1024)
-k_s0_scan(int32_t* __restrict__ rays, uint32_t N, uint32_t Mcap, int32_t* __restrict__ counters) {
+k_s0_scan(int32_t* __restrict__ rays, uint32_t N, uint32_t Mcap, int32_t* __restrict__ counters, int32_t* __restrict__ ray_ctl,
+          uint32_t num_points) {
     __shared__ uint32_t warp_tot[32];
-    __shared__ uint32_t carry_s;
+    __shared__ uint32_t carry_s, n_s;
     const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (threadIdx.x == 0) carry_s = 0;
+    if (threadIdx.x == 0) { carry_s = 0; n_s = ray_count(ray_ctl, N); }       // read before thread 0 rewrites ray_ctl[0] below
     __syncthreads();
+    const uint32_t n_act = n_s;
     for (uint32_t base = 0; base < N; base += 1024) {
         const uint32_t i = base + threadIdx.x;
         const uint32_t v = i < N ? (uint32_t)rays[2 * i + 1] : 0u;
@@ -184,12 +203,23 @@ k_s0_scan(int32_t* __restrict__ rays, uint32_t N, uint32_t Mcap, int32_t* __rest
         // persistent capacity accounting (never reset by the march): steps that overflowed the sample slab, largest M seen
         if (M > Mcap) counters[13] += 1;
         counters[14] = max(counters[14], (int32_t)M);
+        if (ray_ctl) {
+            counters[16] = (int32_t)n_act;
+            uint32_t next = n_act;
+            if (M > 0) {
+                const double want = rint(__dmul_rn(__ddiv_rn((double)num_points, (double)M), (double)n_act));
+                if (want > (double)N) ray_ctl[1] += 1;
+                ray_ctl[2] = max(ray_ctl[2], (int32_t)fmin(want, 2147483647.0));
+                next = (uint32_t)fmin(fmax(want, 1.0), (double)N);
+            }
+            ray_ctl[0] = (int32_t)next;
+        }
     }
-    // part boundaries (n2m_common.cuh part_range): sample offset of the first ray of every eighth of the batch
+    // part boundaries (n2m_common.cuh part_range): sample offset of the first active ray of every eighth of the batch
     if (threadIdx.x <= kPartSlots) {
         const uint32_t e = threadIdx.x;
-        const uint32_t first = part_first_ray(N, e);
-        const uint32_t off = (e == kPartSlots || first >= N) ? M : (uint32_t)rays[2 * first];
+        const uint32_t first = part_first_ray(n_act, e);
+        const uint32_t off = (e == kPartSlots || first >= n_act) ? M : (uint32_t)rays[2 * first];
         counters[4 + e] = (int32_t)min(min(off, M), Mcap);
     }
 }
@@ -534,13 +564,22 @@ __device__ __forceinline__ float entropy_bits(float w, float& dH) {
     return -wc * l1 - (1.0f - wc) * l0;
 }
 
+template <bool ADAPTIVE>
 __global__ void __launch_bounds__(128)
 k_s0_composite_loss(n2m_s0_params p, const float4* __restrict__ out, const float4* __restrict__ recs,
                     const int32_t* __restrict__ rays, const int32_t* __restrict__ counters, uint32_t N,
                     const float* __restrict__ gt, const float* __restrict__ bg, const float* __restrict__ loss_scale,
                     float4* __restrict__ dout, float* __restrict__ image, float* __restrict__ weights_sum,
-                    float* __restrict__ depth, float* __restrict__ loss_out, uint32_t ray_lo, uint32_t ray_hi) {
-    // rays [ray_lo, ray_hi) of the N-ray batch (a part of the batch, n2m_common.cuh part_range); all means stay over N
+                    float* __restrict__ depth, float* __restrict__ loss_out, const int32_t* __restrict__ active, uint32_t lo,
+                    uint32_t hi) {
+    // rays [lo, hi) of the N-ray batch (a part of the batch, n2m_common.cuh part_range).  ADAPTIVE: the batch is its first n = *active
+    // rays (the count the march recorded) and this launch takes rays [n*lo/8, n*hi/8).  All means are over the batch's rays
+    uint32_t n_act = N, ray_lo = lo, ray_hi = hi;
+    if (ADAPTIVE) {
+        n_act = ray_count(active, N);
+        ray_lo = part_first_ray(n_act, lo);
+        ray_hi = part_first_ray(n_act, hi);
+    }
     const uint32_t n = ray_lo + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5);
     const uint32_t lane = threadIdx.x & 31;
     if (n >= ray_hi) return;
@@ -590,7 +629,7 @@ k_s0_composite_loss(n2m_s0_params p, const float4* __restrict__ out, const float
     }
     const float e0 = pr - t0, e1 = pg - t1, e2 = pb - t2;
     float my_loss = (e0 * e0 + e1 * e1 + e2 * e2) * (1.0f / 3.0f);
-    const float invN = 1.0f / (float)N;
+    const float invN = 1.0f / (float)n_act;
     const float sc = loss_scale[0] * invN;
     const float gi0 = sc * (2.0f / 3.0f) * e0, gi1 = sc * (2.0f / 3.0f) * e1, gi2 = sc * (2.0f / 3.0f) * e2;
     float gws = -(gi0 * b0 + gi1 * b1 + gi2 * b2);          // pred = image + (1 - ws) * bg
@@ -852,20 +891,20 @@ int n2m_s0_unpack_grads(const void* gtable, uint32_t rows, const float* loss_sca
 
 int n2m_s0_march(const n2m_s0_params* p, const float* rays_o, const float* rays_d, const float* aabb,
                  const float* cam_near_far, const uint8_t* bitfield, const float* noises, uint32_t N, int32_t* rays,
-                 int32_t* counters, float* tbuf, void* recs, uint32_t Mcap, n2m_stream_t stream) {
+                 int32_t* counters, float* tbuf, void* recs, uint32_t Mcap, int32_t* ray_ctl, uint32_t num_points,
+                 n2m_stream_t stream) {
     N2M_REQUIRE(p && rays && counters, "s0_march", "null pointer");
     cudaStream_t st = as_stream(stream);
     if (N == 0) { cudaMemsetAsync(counters, 0, 4 * sizeof(int32_t), st); return 0; }
     N2M_REQUIRE(rays_o && rays_d && aabb && bitfield && noises && tbuf && recs, "s0_march", "null pointer");
     N2M_REQUIRE(p->max_steps > 0 && p->grid_size > 0 && p->cascades > 0, "s0_march", "bad params");
-    if (g_serial_march)
-        k_s0_count<<<div_up(N, 128u), 128, 0, st>>>(rays_o, rays_d, aabb, cam_near_far, bitfield, noises, *p, N, rays,
-                                                     reinterpret_cast<float2*>(tbuf));
-    else
-        k_s0_count_warp<<<div_up(N * 32u, 128u), 128, 0, st>>>(rays_o, rays_d, aabb, cam_near_far, bitfield, noises, *p, N, rays,
-                                                                reinterpret_cast<float2*>(tbuf));
+    N2M_REQUIRE(!ray_ctl || num_points > 0, "s0_march", "adaptive ray count needs num_points > 0");
+    auto count = g_serial_march ? (ray_ctl ? k_s0_count<true> : k_s0_count<false>)
+                                : (ray_ctl ? k_s0_count_warp<true> : k_s0_count_warp<false>);
+    count<<<g_serial_march ? div_up(N, 128u) : div_up(N * 32u, 128u), 128, 0, st>>>(rays_o, rays_d, aabb, cam_near_far, bitfield, noises,
+                                                                                   *p, N, ray_ctl, rays, reinterpret_cast<float2*>(tbuf));
     if (int e = check_launch("s0_march(count)")) return e;
-    k_s0_scan<<<1, 1024, 0, st>>>(rays, N, Mcap, counters);
+    k_s0_scan<<<1, 1024, 0, st>>>(rays, N, Mcap, counters, ray_ctl, num_points);
     if (int e = check_launch("s0_march(scan)")) return e;
     k_s0_records<<<div_up(N * 32u, 256u), 256, 0, st>>>(rays, reinterpret_cast<const float2*>(tbuf), N, p->max_steps, Mcap,
                                                         static_cast<float4*>(recs));
@@ -981,17 +1020,25 @@ int n2m_s0_tv_random(const n2m_s0_params* p, const int32_t* counters, const void
 int n2m_s0_composite_loss(const n2m_s0_params* p, const void* out, const void* recs, const int32_t* rays,
                           const int32_t* counters, uint32_t N, uint32_t Mcap, const float* gt, const float* bg,
                           const float* loss_scale, void* dout, float* image, float* weights_sum, float* depth,
-                          float* loss_out, uint32_t part, uint32_t nparts, n2m_stream_t stream) {
+                          float* loss_out, const int32_t* active_rays, uint32_t part, uint32_t nparts, n2m_stream_t stream) {
     (void)Mcap;
     if (N == 0) return 0;
     N2M_REQUIRE(p && out && recs && rays && counters && gt && bg && loss_scale && dout && image && weights_sum && depth && loss_out,
                 "s0_composite_loss", "null pointer");
     N2M_REQUIRE(valid_parts(part, nparts), "s0_composite_loss", "nparts must be 1, 2, 4 or 8 and part < nparts");
-    const uint32_t ray_lo = part_first_ray(N, part * kPartSlots / nparts), ray_hi = part_first_ray(N, (part + 1) * kPartSlots / nparts);
+    const uint32_t e0 = part * kPartSlots / nparts, e1 = (part + 1) * kPartSlots / nparts;
+    if (active_rays) {
+        // the part's rays are known on the device only: the grid covers the largest part any n <= N can give, ceil(N / nparts)
+        k_s0_composite_loss<true><<<div_up(div_up(N, nparts) * 32u, 128u), 128, 0, as_stream(stream)>>>(
+            *p, static_cast<const float4*>(out), static_cast<const float4*>(recs), rays, counters, N, gt, bg, loss_scale,
+            static_cast<float4*>(dout), image, weights_sum, depth, loss_out, active_rays, e0, e1);
+        return check_launch("s0_composite_loss");
+    }
+    const uint32_t ray_lo = part_first_ray(N, e0), ray_hi = part_first_ray(N, e1);
     if (ray_hi == ray_lo) return 0;
-    k_s0_composite_loss<<<div_up((ray_hi - ray_lo) * 32u, 128u), 128, 0, as_stream(stream)>>>(
+    k_s0_composite_loss<false><<<div_up((ray_hi - ray_lo) * 32u, 128u), 128, 0, as_stream(stream)>>>(
         *p, static_cast<const float4*>(out), static_cast<const float4*>(recs), rays, counters, N, gt, bg, loss_scale,
-        static_cast<float4*>(dout), image, weights_sum, depth, loss_out, ray_lo, ray_hi);
+        static_cast<float4*>(dout), image, weights_sum, depth, loss_out, nullptr, ray_lo, ray_hi);
     return check_launch("s0_composite_loss");
 }
 

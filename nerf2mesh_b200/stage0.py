@@ -43,14 +43,14 @@ _lib.register({
     "n2m_s0_pack_tables": [P, P, U, P, P, P],
     "n2m_s0_unpack_tables": [P, P, U, P, P, P],
     "n2m_s0_unpack_grads": [P, U, P, P, P, P],
-    "n2m_s0_march": [PP, P, P, P, P, P, P, U, P, P, P, P, U, P],
+    "n2m_s0_march": [PP, P, P, P, P, P, P, U, P, P, P, P, U, P, U, P],
     "n2m_s0_encode_fwd": [PP, P, P, U, P, P, P, P, P, U, U, P],
     "n2m_s0_encode_points": [PP, P, P, P, U, P, P, P, P],
     "n2m_s0_grid_points": [U, U, U, F, P, P, P],
     "n2m_s0_grid_update": [P, U, F, P, P],
     "n2m_s0_packbits_dev": [P, U, P, F, P, P],
     "n2m_s0_mlp_fwd": [PP, P, P, U, P, P, P, U, U, P],
-    "n2m_s0_composite_loss": [PP, P, P, P, P, U, U, P, P, P, P, P, P, P, P, U, U, P],
+    "n2m_s0_composite_loss": [PP, P, P, P, P, U, U, P, P, P, P, P, P, P, P, P, U, U, P],
     "n2m_s0_mlp_bwd": [PP, P, P, P, U, P, P, P, P, U, U, P],
     "n2m_s0_encode_bwd": [PP, P, P, U, P, P, P, P, P, P, P, U, U, P],
     "n2m_s0_adam_head": [P, P, P],
@@ -83,7 +83,7 @@ class Stage0Config:
     def __init__(self, bound=1.0, contract=False, dt_gamma=0.0, max_steps=1024, grid_size=128, min_near=0.05,
                  T_thresh=1e-4, num_levels=16, base_resolution=16, log2_hashmap_size=19, lambda_mask=0.1,
                  lambda_specular=1e-5, lambda_tv=1e-8, lambda_entropy=0.0, lr=1e-2, eps=1e-15, max_samples=None, num_rays=4096,
-                 loss_scale=65536.0):
+                 loss_scale=65536.0, adaptive_num_rays=False, num_points=2 ** 18, max_rays=None):
         self.real_bound = float(bound)
         self.contract = bool(contract)
         self.bound = 2.0 if contract else float(bound)          # renderer.py:74-80
@@ -97,6 +97,16 @@ class Stage0Config:
         self.lambda_entropy = float(lambda_entropy)          # main.py --lambda_entropy (garden recipe: 1e-3)
         self.lr, self.eps = float(lr), float(eps)
         self.num_rays = int(num_rays)
+        # --adaptive_num_rays (main.py:68-69,129-135): after every step the next batch takes round(num_points / M * n) rays, decided
+        # on the device by the march (include/n2m_b200_fused.h ray_ctl).  The first step takes num_rays; the per-ray buffers are max_rays
+        # wide and every step() is handed max_rays rows, of which the trainer uses the first n.
+        self.adaptive_num_rays = bool(adaptive_num_rays)
+        self.num_points = int(num_points)
+        self.max_rays = (int(max_rays) if max_rays else 4 * self.num_rays) if self.adaptive_num_rays else self.num_rays
+        if self.adaptive_num_rays and self.num_points <= 0:
+            raise ValueError(f"num_points must be positive, got {self.num_points}")
+        if self.adaptive_num_rays and self.max_rays < self.num_rays:
+            raise ValueError(f"max_rays ({self.max_rays}) must be at least num_rays ({self.num_rays})")
         # sample capacity of the per-step buffers.  The reference allocates exactly M samples per step (raymarching.py:232-238)
         # and never drops a ray; here a step whose M exceeds the capacity renders the rays that do not fit (the LAST rays of the
         # batch) as background without gradient -- counted on the device (counters[13], [14]); Stage0Trainer.check_capacity()
@@ -114,7 +124,7 @@ class _Slot:
         self.gt = torch.zeros(N, 4, device=dev); self.bg = torch.zeros(N, 3, device=dev)
         self.noises = torch.zeros(N, device=dev)
         self.rays = torch.zeros(N, 2, dtype=torch.int32, device=dev)
-        self.counters = torch.zeros(16, dtype=torch.int32, device=dev)    # include/n2m_b200_fused.h: [4..12] part boundaries
+        self.counters = torch.zeros(17, dtype=torch.int32, device=dev)    # include/n2m_b200_fused.h: [4..12] part boundaries, [16] n
         self.tbuf = torch.empty(N * max_steps * 2, device=dev)
         self.recs = torch.zeros(Mc, 4, device=dev)
         self.cam_nf = torch.zeros(N, 2, device=dev)                      # per-ray (near, far) clamp, renderer.py:689-691
@@ -137,6 +147,11 @@ class _Slot:
 
 
 class Stage0Trainer:
+    # adaptive ray count (Stage0Config.adaptive_num_rays): the device-resident control block the march reads and rewrites
+    adaptive = False
+    ray_ctl = None
+    _ray_ctl_undo = None        # ray_ctl as it was before the side-stream march of a prefetched batch (see drop_prefetch)
+
     def __init__(self, cfg: Stage0Config, device="cuda", seed=0):
         self.cfg = cfg
         self.device = torch.device(device)
@@ -170,8 +185,12 @@ class Stage0Trainer:
         self.aabb = torch.tensor([-b, -b, -b, b, b, b], dtype=torch.float32, device=dev)
         # ---- per-batch buffers: two slots, so the (parameter-independent) march of batch i+1 can run on a side
         # stream while batch i is in encode / MLP / scatter / Adam ----
-        N, Mc = c.num_rays, c.max_samples
+        N, Mc = c.max_rays, c.max_samples
         self.N, self.Mcap = N, Mc
+        if c.adaptive_num_rays:
+            self.adaptive = True
+            self.ray_ctl = torch.tensor([c.num_rays, 0, 0, 0], dtype=torch.int32, device=dev)     # include/n2m_b200_fused.h ray_ctl
+            self._ray_ctl_undo = torch.zeros_like(self.ray_ctl)
         self.slots = [_Slot(N, Mc, c.max_steps, dev) for _ in range(2)]
         self.cur = 0
         self._prefetched = None                 # slot index holding an already staged + marched batch
@@ -431,10 +450,13 @@ class Stage0Trainer:
     def _pp(self):
         return ctypes.byref(self.params)
 
-    def march(self):
+    def march(self, all_rays=False):
+        """`all_rays`: march every row of the buffers whatever the adaptive ray count (evaluation)."""
+        adaptive = self.adaptive and not all_rays
         call("n2m_s0_march", self._pp(), ptr(self.rays_o), ptr(self.rays_d), ptr(self.aabb),
              ptr(self.slots[self.cur].cam_nf) if self.use_cam_near_far else None, ptr(self.density_bitfield),
-             ptr(self.noises), self.N, ptr(self.rays), ptr(self.counters), ptr(self.tbuf), ptr(self.recs), self.Mcap, stream())
+             ptr(self.noises), self.N, ptr(self.rays), ptr(self.counters), ptr(self.tbuf), ptr(self.recs), self.Mcap,
+             ptr(self.ray_ctl) if adaptive else None, self.cfg.num_points if adaptive else 0, stream())
 
     def encode_fwd(self, part=0, nparts=1):
         call("n2m_s0_encode_fwd", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
@@ -444,10 +466,11 @@ class Stage0Trainer:
         call("n2m_s0_mlp_fwd", self._pp(), ptr(self.enc_tiles), ptr(self.counters), self.Mcap, ptr(self.wpack), ptr(self.out),
              self.loss_acc.data_ptr() + 4, part, nparts, stream())
 
-    def composite_loss(self, part=0, nparts=1):
+    def composite_loss(self, part=0, nparts=1, all_rays=False):
+        active = self.counters.data_ptr() + 4 * 16 if self.adaptive and not all_rays else None      # counters[16]: the batch's n
         call("n2m_s0_composite_loss", self._pp(), ptr(self.out), ptr(self.recs), ptr(self.rays), ptr(self.counters), self.N, self.Mcap,
              ptr(self.gt), ptr(self.bg), ptr(self.opt_state), ptr(self.dout), ptr(self.image), ptr(self.weights_sum), ptr(self.depth),
-             ptr(self.loss_acc), part, nparts, stream())
+             ptr(self.loss_acc), active, part, nparts, stream())
 
     def mlp_bwd(self, part=0, nparts=1):
         call("n2m_s0_mlp_bwd", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.Mcap, ptr(self.wpack),
@@ -635,6 +658,8 @@ class Stage0Trainer:
           (which do not depend on the parameters) are enqueued on a side stream and overlap this step's
           compute.  The following step() call must then pass that same batch (its copy and march are skipped).
         * `grad_sync`: callable run between backward and optimizer (data-parallel gradient all-reduce).
+        * adaptive ray count (`cfg.adaptive_num_rays`): every batch has `max_rays` (= self.N) rows; the step uses the first n, the count
+          the previous march left in `ray_ctl[0]` (recorded in the slot's counters[16]); rows >= n are never read.
         No host sync happens here; read `loss_acc` / `counters` afterwards."""
         main = torch.cuda.current_stream()
         if self._prefetched is not None:
@@ -665,8 +690,12 @@ class Stage0Trainer:
             if split:
                 ev_mid = torch.cuda.Event(); ev_mid.record(main)
 
+        ev_marched = None
         if not marched:
             self._run("march", self.march, use_graph)
+            if next_batch is not None and self.adaptive and not split:
+                # the next batch's march reads the ray count this march's scan writes (ray_ctl[0])
+                ev_marched = torch.cuda.Event(); ev_marched.record(main)
         if grad_sync is None:
             if split:
                 self._run("compute_sg", self._compute_sg, use_graph)
@@ -701,11 +730,15 @@ class Stage0Trainer:
             if self._ev_done[nxt] is not None:
                 side.wait_event(self._ev_done[nxt])              # slot `nxt` was last read by the previous step
             side.wait_event(ev_start)
+            if ev_marched is not None:
+                side.wait_event(ev_marched)
             keep = self.cur
             with torch.cuda.stream(side):
                 self.slots[nxt].load(*next_batch)
                 if ev_mid is not None:
                     side.wait_event(ev_mid)
+                if self.adaptive:
+                    self._ray_ctl_undo.copy_(self.ray_ctl)          # a dropped prefetch restores it (drop_prefetch)
                 self.cur = nxt
                 self._run("march", self.march, use_graph)
                 self.cur = keep
@@ -875,8 +908,9 @@ class Stage0Trainer:
         slot = self.slots[self.cur]
         zeros3 = torch.zeros(self.N, 3, device=self.device)
         bg = torch.full((self.N, 3), float(bg_color), device=self.device) if not torch.is_tensor(bg_color) else None
-        for a in range(0, R, self.N):
-            b = min(R, a + self.N)
+        C = self.cfg.num_rays           # rays per chunk: the sample slab is sized for num_rays, also when the buffers are max_rays wide
+        for a in range(0, R, C):
+            b = min(R, a + C)
             n = b - a
             ro = torch.zeros(self.N, 3, device=self.device); rd = torch.ones(self.N, 3, device=self.device)
             ro[:n] = rays_o[a:b]; rd[:n] = rays_d[a:b]
@@ -886,7 +920,7 @@ class Stage0Trainer:
                 bgc = torch.ones(self.N, 3, device=self.device); bgc[:n] = bg_color[a:b]
             slot.load(ro, rd, zeros3, bg if bg is not None else bgc, torch.zeros(self.N, device=self.device))
             self.loss_acc.zero_()
-            self.march(); self.encode_fwd(); self.mlp_fwd(); self.composite_loss()
+            self.march(all_rays=True); self.encode_fwd(); self.mlp_fwd(); self.composite_loss(all_rays=True)
             img[a:b] = self.image[:n]; ws[a:b] = self.weights_sum[:n]; dep[a:b] = self.depth[:n]
         return img, ws, dep
 
@@ -905,6 +939,18 @@ class Stage0Trainer:
                 self._resize_samples(new_cap)
         return over, max_m
 
+    def check_rays(self):
+        """(host sync) adaptive ray count -> (steps whose requested count was clamped to max_rays since the last call, largest count
+        requested since the last call, ray count of the next march).  Without adaptive mode (0, num_rays, num_rays), no sync.
+        Drops a prefetched batch first, as check_capacity() does: its staged march has counted a request of a step not yet run."""
+        if not self.adaptive:
+            return 0, self.N, self.N
+        self.drop_prefetch()
+        torch.cuda.synchronize()
+        nxt, clamped, largest = (int(v) for v in self.ray_ctl[:3].tolist())
+        self.ray_ctl[1:3] = 0
+        return clamped, largest, nxt
+
     def _resize_samples(self, Mc):
         dev = self.device
         self.Mcap = self.cfg.max_samples = int(Mc)
@@ -918,10 +964,14 @@ class Stage0Trainer:
         self._graphs = {}
 
     def drop_prefetch(self):
-        """Forget a batch staged by `next_batch=` (e.g. when the caller changes its batch sequence)."""
+        """Forget a batch staged by `next_batch=` (e.g. when the caller changes its batch sequence).  With the adaptive ray count the
+        dropped march has already written the count after its own batch and counted its request: the control block is put back as it
+        was before that march, so the next step takes the count the reference would and the clamp counts stay those of the steps run."""
         if self._side is not None:
             self._side.synchronize()
         if self._prefetched is not None:
+            if self.adaptive:
+                self.ray_ctl.copy_(self._ray_ctl_undo)
             self.cur = self._prefetched      # keep the slot alternation in phase (graphs are captured per slot)
         self._prefetched = None
 

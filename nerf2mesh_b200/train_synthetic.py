@@ -51,6 +51,10 @@ def main(argv=None):
     ap.add_argument("--train_res", type=int, default=400, help="resolution of the device-resident training views")
     ap.add_argument("--samples_per_ray", type=int, default=512,
                     help="sample-slab capacity per ray; the cold-start occupancy grid marches far more samples than a converged one")
+    ap.add_argument("--adaptive_num_rays", action="store_true",
+                    help="resize every batch to march about --num_points samples, as the reference's -O preset does (main.py:68-69); "
+                         "batches start at --num_rays and are drawn with 4 x --num_rays rows, of which the trainer uses the first n")
+    ap.add_argument("--num_points", type=int, default=2 ** 18, help="target samples per step with --adaptive_num_rays")
     args = ap.parse_args(argv)
 
     torch.manual_seed(args.seed)
@@ -59,8 +63,10 @@ def main(argv=None):
     poses = S.orbit_cameras(100, seed=0)
     test_poses = S.orbit_cameras(args.eval_views, seed=12345)
     intr = S.lego_intrinsics()
-    cfg = Stage0Config(bound=1.0, num_rays=args.num_rays, max_samples=args.num_rays * args.samples_per_ray)
+    cfg = Stage0Config(bound=1.0, num_rays=args.num_rays, max_samples=args.num_rays * args.samples_per_ray,
+                       adaptive_num_rays=args.adaptive_num_rays, num_points=args.num_points)
     tr = Stage0Trainer(cfg, seed=args.seed)
+    rows = tr.N                   # rows per batch: num_rays, or max_rays with the adaptive ray count
     # cold start as the reference: empty density grid => first update marks everything with sigma > mean
     tr.density_grid.zero_()
     g = torch.Generator().manual_seed(args.seed + 1)
@@ -79,16 +85,16 @@ def main(argv=None):
         gd = torch.Generator(device=dev).manual_seed(args.seed + 1)
 
         def batch():
-            ro, rd, gt = sampler.sample(args.num_rays, generator=gd)
-            bg = torch.rand(args.num_rays, 3, device=dev, generator=gd)
-            noises = torch.rand(args.num_rays, device=dev, generator=gd)
+            ro, rd, gt = sampler.sample(rows, generator=gd)
+            bg = torch.rand(rows, 3, device=dev, generator=gd)
+            noises = torch.rand(rows, device=dev, generator=gd)
             return ro, rd, gt, bg, noises
     else:
         def batch():
-            ro, rd, _, _ = S.sample_rays(poses, intr, 800, 800, args.num_rays, g)
+            ro, rd, _, _ = S.sample_rays(poses, intr, 800, 800, rows, g)
             gt = S.render_bricks(ro, rd, bricks)
-            bg = torch.rand(args.num_rays, 3, generator=g)
-            noises = torch.rand(args.num_rays, generator=g)
+            bg = torch.rand(rows, 3, generator=g)
+            noises = torch.rand(rows, generator=g)
             return tuple(t.pin_memory() for t in (ro, rd, gt, bg, noises))
 
     t0 = time.time()
@@ -102,7 +108,8 @@ def main(argv=None):
         if it % 250 == 0 or it == args.iters - 1:
             torch.cuda.synchronize()
             m = int(tr.counters[1].item())
-            log.append({"it": it, "loss": tr.read_loss(), "samples": m, "overflow": int(tr.counters[2].item()),
+            n = int(tr.counters[16].item()) if args.adaptive_num_rays else args.num_rays
+            log.append({"it": it, "loss": tr.read_loss(), "n": n, "samples": m, "overflow": int(tr.counters[2].item()),
                         "occ": float((tr.density_bitfield != 0).float().mean().item()), "loss_scale": float(tr.opt_state[0].item())})
             print(log[-1], flush=True)
     torch.cuda.synchronize()

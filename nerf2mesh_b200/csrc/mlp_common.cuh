@@ -80,9 +80,10 @@ __device__ __forceinline__ void row_cols(const float (&acc)[2][N / 2], float (&v
     }
 }
 
-// 128 x NCOL accumulator -> optional ReLU / mask -> fp16 128-row chunk-major tile.  mask_tile != nullptr: zero where the fp16
+// 128 x NCOL accumulator -> optional ReLU / mask -> fp16 128-row chunk-major tile.  mask_tile != nullptr: +0 where the fp16
 // activation stored there is <= 0.  ReLU and the mask are applied on packed half2 values, bit-identical to the fp32 formulation
-// (rounding to fp16 commutes with max(., 0) and with zeroing).
+// (rounding to fp16 commutes with max(., 0) and with zeroing).  The mask is a select (bitwise AND with __hgt2_mask), as the
+// backward of torch's relu (threshold_backward) is: a multiply by 0 would turn a masked gradient that overflowed fp16 into NaN.
 // Shared-memory accesses by 32-bit shared-window address: one base register per tile and immediate offsets, where generic
 // pointers would take a 64-bit address register pair per access of an unrolled epilogue.
 __device__ __forceinline__ void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" :: "r"(addr), "r"(v) : "memory"); }
@@ -107,8 +108,9 @@ __device__ __forceinline__ void epi_store(const float (&acc)[2][NCOL / 2], uint8
             const uint32_t off = wg::tile_off(64u * hh + 8u * ((i >> 1) & 1), 8u * (i >> 2), kTile);
             __half2 h = __floats2half2_rn(acc[hh][i], acc[hh][i + 1]);
             if (RELU) h = __hmax2(h, zero2);
-            if (mask_tile) h = __hmul2(h, __hgt2(bits_h2(lds32(m + off)), zero2));
-            sts32(t + off, h2_bits(h));
+            uint32_t hb = h2_bits(h);
+            if (mask_tile) hb &= __hgt2_mask(bits_h2(lds32(m + off)), zero2);
+            sts32(t + off, hb);
         }
 }
 

@@ -27,6 +27,38 @@
  *   n2m_mark_seen_faces : rast [num_pixels,4] f32 of one view -> seen[(long)rast.w - 1] = 1 (caller zeroes seen [F] u8).  The index of an
  *                         uncovered pixel is -1, which the reference's torch indexing wraps to the last face: face F-1 counts as seen
  *                         whenever the view has an empty pixel (mark_unseen_triangles, renderer.py:947-981, kept as is).
+ *
+ * Mesh clean-up (remove_masked_trigs and clean_mesh(..., remesh=False) of meshutils.py:63-93,146-188, pymeshlab in the reference;
+ * csrc/meshclean.cu; Python: mesh.remove_masked_faces, mesh.clean_mesh).  The steps never move the mesh: faces are dropped through
+ * fkeep [F] u8, merged and split vertices are re-indexed in place in tri [F,3] i32, and the caller compacts once with n2m_rsv_emit.  Power-
+ * of-two tables and sort buffers are the caller's; each entry initialises what it documents.
+ *   n2m_clean_mark_verts    : vflag[v] = 1 for every corner of a face with fkeep set (fkeep NULL: every face); caller zeroes vflag [V] u8
+ *   n2m_clean_dilate        : one selection dilation: vsel [V] u8 |= the corners of kept faces, then fkeep[f] = 1 where a corner is selected
+ *   n2m_clean_bbox          : bbox [6] u32 = order-preserving keys of the min / max xyz over the vertices with vflag set (initialised here)
+ *   n2m_clean_merge_bin     : close-vertex merge, radius r = v_pct / 100 * diag / 10 (float64, diag of bbox): vbucket [V] i32 = the
+ *                             bucket of the vertex's cell of size r in a table of nbuckets, bucket_count [nbuckets] i32 += 1 (caller zeroes)
+ *   n2m_clean_merge_fill    : cursor = EXCLUSIVE prefix sum of bucket_count (advanced here) -> items [V] i32 grouped by bucket
+ *   n2m_clean_merge_round   : one decision round (round = 1, 2, ...) over the flagged, undecided vertices; decided [V] i32 zeroed by the
+ *                             caller before round 1, target [V] i32 = the vertex's leader once decided; pending [1] i32 = 1 (caller
+ *                             zeroes) while a vertex is still undecided.  bucket_start [nbuckets+1] i32: inclusive prefix after a 0.
+ *                             Leader rule: i leads unless a leader j < i lies within r, dx*dx + dy*dy + dz*dz <= r*r in float64
+ *   n2m_clean_merge_apply   : tri <- target[tri] for kept faces; a face repeating an index is dropped
+ *   n2m_clean_dup_null      : drop the kept faces whose unordered vertex triple a lower kept face has, and those whose float64
+ *                             cross(b - a, c - a) is the zero vector; table [nslots >= 2F] i32 and slot_of [F] i32 are scratch
+ *   n2m_clean_edge_table    : table [nslots >= 6F] i32 of the kept faces' unordered edges (slot value = lowest face-edge 3f+k with the
+ *                             edge), slot_of [3F] i32 = the slot of face-edge 3f+k (edge from corner k to corner k+1)
+ *   n2m_clean_components    : edge-connected components of the kept faces over that table; drop a component whose bbox diagonal is
+ *                             < min_d / 100 * diag (diag of bbox; min_d > 0) or whose face count is < min_f (min_f > 0).  parent,
+ *                             label, count [F] i32, cmin, cmax [3F] u32 are scratch
+ *   n2m_clean_nm_edges      : the kept faces with an edge of > 2 kept faces, visited by (float64 area, face index); a face goes when one
+ *                             of its edges still has > 2 kept faces.  ecount [nslots] i32, ncand [1] i32, keys [capacity] u64,
+ *                             vals [capacity] i32 are scratch (capacity a power of two >= F)
+ *   n2m_clean_nm_verts_find : fans of every vertex (kept faces joined through an edge at the vertex); nextra [1] i32 = the number of fans
+ *                             that do not hold the vertex's lowest face, cnew [3F] i32 numbers them in (vertex, lowest face) order.
+ *                             emin [nslots], cparent, clabel [3F], vmin [V] i32, keys / vals [capacity >= 3F] are scratch; clabel (each
+ *                             corner's fan root) and vmin feed n2m_clean_nm_verts_apply
+ *   n2m_clean_nm_verts_apply: the corners of those fans take vertex V + cnew, ext_vertices [V + nextra, 3] f32 rows V.. get the copies'
+ *                             positions (the caller copies rows 0..V-1)
  */
 #ifndef N2M_B200_MESH_H
 #define N2M_B200_MESH_H
@@ -49,6 +81,31 @@ int n2m_rsv_count(const uint8_t* removed, uint32_t V, const int32_t* tri, uint32
 int n2m_rsv_emit(const float* vertices, uint32_t V, const int32_t* tri, uint32_t F, const uint8_t* vkeep, const uint8_t* fkeep,
                  const int32_t* voff, const int32_t* foff, float* out_v, int32_t* out_f, n2m_stream_t stream);
 int n2m_mark_seen_faces(const float* rast, uint32_t num_pixels, uint32_t F, uint8_t* seen, n2m_stream_t stream);
+
+int n2m_clean_mark_verts(const int32_t* tri, uint32_t F, const uint8_t* fkeep, uint8_t* vflag, n2m_stream_t stream);
+int n2m_clean_dilate(const int32_t* tri, uint32_t F, uint8_t* fkeep, uint8_t* vsel, n2m_stream_t stream);
+int n2m_clean_bbox(const float* vertices, uint32_t V, const uint8_t* vflag, uint32_t* bbox, n2m_stream_t stream);
+int n2m_clean_merge_bin(const float* vertices, uint32_t V, const uint8_t* vflag, const uint32_t* bbox, double v_pct, uint32_t nbuckets,
+                        int32_t* bucket_count, int32_t* vbucket, n2m_stream_t stream);
+int n2m_clean_merge_fill(uint32_t V, const uint8_t* vflag, const int32_t* vbucket, int32_t* cursor, int32_t* items, n2m_stream_t stream);
+int n2m_clean_merge_round(const float* vertices, uint32_t V, const uint8_t* vflag, const uint32_t* bbox, double v_pct, uint32_t nbuckets,
+                          const int32_t* bucket_start, const int32_t* items, int32_t round, int32_t* decided, int32_t* target,
+                          int32_t* pending, n2m_stream_t stream);
+int n2m_clean_merge_apply(int32_t* tri, uint32_t F, const int32_t* target, uint8_t* fkeep, n2m_stream_t stream);
+int n2m_clean_dup_null(const float* vertices, const int32_t* tri, uint32_t F, uint8_t* fkeep, uint32_t nslots, int32_t* table,
+                       int32_t* slot_of, n2m_stream_t stream);
+int n2m_clean_edge_table(const int32_t* tri, uint32_t F, const uint8_t* fkeep, uint32_t nslots, int32_t* table, int32_t* slot_of,
+                         n2m_stream_t stream);
+int n2m_clean_components(const float* vertices, const int32_t* tri, uint32_t F, uint8_t* fkeep, const int32_t* table, const int32_t* slot_of,
+                         const uint32_t* bbox, double min_d, uint32_t min_f, int32_t* parent, int32_t* label, int32_t* count, uint32_t* cmin,
+                         uint32_t* cmax, n2m_stream_t stream);
+int n2m_clean_nm_edges(const float* vertices, const int32_t* tri, uint32_t F, uint8_t* fkeep, const int32_t* slot_of, uint32_t nslots,
+                       int32_t* ecount, int32_t* ncand, uint64_t* keys, int32_t* vals, uint32_t capacity, n2m_stream_t stream);
+int n2m_clean_nm_verts_find(const int32_t* tri, uint32_t V, uint32_t F, const uint8_t* fkeep, const int32_t* slot_of, uint32_t nslots,
+                            int32_t* emin, int32_t* cparent, int32_t* clabel, int32_t* vmin, int32_t* nextra, uint64_t* keys, int32_t* vals,
+                            int32_t* cnew, uint32_t capacity, n2m_stream_t stream);
+int n2m_clean_nm_verts_apply(const float* vertices, uint32_t V, int32_t* tri, uint32_t F, const uint8_t* fkeep, const int32_t* clabel,
+                             const int32_t* vmin, const int32_t* cnew, float* ext_vertices, n2m_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -6,15 +6,22 @@ third-party CPU library) with the kernels of csrc/mcubes.cu (C ABI include/n2m_b
     vertices, triangles = marching_cubes(volume, isovalue)      # volume [X,Y,Z] float32 CUDA tensor
     # vertices [V,3] float32 in index coordinates (0 .. X-1), triangles [F,3] int32 -- the form PyMCubes returns (as tensors)
 
-`export_stage0_mesh(trainer, path, resolution)` is the reference's export up to (not including) its CPU clean-up / decimation:
-density volume (Stage0Trainer.density_volume == renderer.py:480-524) -> marching cubes -> `vertices / (resolution - 1) * 2 - 1` (:531) ->
-`mesh_0.ply`.  No CPU fallback: the volume must live on a CUDA device.
+`export_stage0_mesh(trainer, path, resolution)` is the reference's export up to (not including) its decimation: density volume
+(Stage0Trainer.density_volume == renderer.py:480-524) -> marching cubes -> `vertices / (resolution - 1) * 2 - 1` (:531) -> with
+`clean=CleanOptions(...)` the visibility test, remove_masked_faces and clean_mesh -> `mesh_0.ply`.  No CPU fallback: the volume must
+live on a CUDA device.
+
+The reference's pymeshlab post-processing (meshutils.py) is restated as exact rules in csrc/meshclean.cu: `remove_masked_faces`
+(remove_masked_trigs: the faces a mask keeps, dilated along shared vertices) and `clean_mesh` (clean_mesh(..., remesh=False): close-vertex
+merge, duplicate and null faces, small components, non-manifold edges and vertices).  The mesh stays on the device from marching cubes to
+the PLY writer; the host reads back output sizes and the merge's round flags only.  Decimation (decimate_mesh) is not here.
 
 Unbounded scenes (bound > 1, C = 1 + ceil(log2(bound)) cascades) also get one mesh per outer cascade (csrc/cascade.cu):
-`export_outer_meshes(trainer, path, env_reso)` is the non-SDF branch of export_stage0 for cas = 1 .. C-1 (renderer.py:606-672) up to its CPU
-clean-up / decimation -- occupancy volume of density_grid[cas] -> marching cubes at 0.5 -> world coordinates (float64, rounded once) ->
-removal of the centre box and of what lies outside the training AABB -> `mesh_{cas}.ply`.  `mark_unseen_triangles` is the reference's
-visibility test on those meshes, `load_stage0_meshes` picks every cascade's mesh up again for stage 1.
+`export_outer_meshes(trainer, path, env_reso)` is the non-SDF branch of export_stage0 for cas = 1 .. C-1 (renderer.py:606-672) up to its
+decimation -- occupancy volume of density_grid[cas] -> marching cubes at 0.5 -> world coordinates (float64, rounded once) -> removal of
+the centre box and of what lies outside the training AABB -> with `clean=` clean_mesh and the visibility test -> `mesh_{cas}.ply`.
+`mark_unseen_triangles` is the reference's visibility test on those meshes, `load_stage0_meshes` picks every cascade's mesh up again for
+stage 1.
 """
 import ctypes
 import os
@@ -38,6 +45,19 @@ _lib.register({
     "n2m_rsv_count": [P, U, P, U, P, P, P],
     "n2m_rsv_emit": [P, U, P, U, P, P, P, P, P, P, P],
     "n2m_mark_seen_faces": [P, U, U, P, P],
+    "n2m_clean_mark_verts": [P, U, P, P, P],
+    "n2m_clean_dilate": [P, U, P, P, P],
+    "n2m_clean_bbox": [P, U, P, P, P],
+    "n2m_clean_merge_bin": [P, U, P, P, D, U, P, P, P],
+    "n2m_clean_merge_fill": [U, P, P, P, P, P],
+    "n2m_clean_merge_round": [P, U, P, P, D, U, P, P, ctypes.c_int32, P, P, P, P],
+    "n2m_clean_merge_apply": [P, U, P, P, P],
+    "n2m_clean_dup_null": [P, P, U, P, U, P, P, P],
+    "n2m_clean_edge_table": [P, U, P, U, P, P, P],
+    "n2m_clean_components": [P, P, U, P, P, P, P, D, U, P, P, P, P, P, P],
+    "n2m_clean_nm_edges": [P, P, U, P, P, U, P, P, P, P, U, P],
+    "n2m_clean_nm_verts_find": [P, U, U, P, P, U, P, P, P, P, P, P, P, P, U, P],
+    "n2m_clean_nm_verts_apply": [P, U, P, U, P, P, P, P, P, P],
 })
 
 _tables = {}
@@ -103,16 +123,21 @@ def read_ply(path):
     return v.copy(), faces["i"].copy()
 
 
-def export_stage0_mesh(trainer, save_path, resolution=512, density_thresh=10.0):
-    """NeRFRenderer.export_stage0 for the inner region up to its CPU post-processing (renderer.py:471-531,543-544): density volume ->
-    marching cubes at min(mean_density, density_thresh) -> world coordinates -> `<save_path>/mesh_0.ply`.  Returns (vertices, triangles)
-    on the device.  Cleaning / decimation (clean_mesh, decimate_mesh: pymeshlab) stay the caller's CPU code; the outer-region meshes of an
-    unbounded scene come from `export_outer_meshes`."""
+def export_stage0_mesh(trainer, save_path, resolution=512, density_thresh=10.0, *, clean=None):
+    """NeRFRenderer.export_stage0 for the inner region up to its decimation (renderer.py:471-544): density volume -> marching cubes at
+    min(mean_density, density_thresh) -> world coordinates -> with `clean` (a CleanOptions): the visibility test and remove_masked_faces
+    when it carries views, then clean_mesh(repair=True) (:531-537) -> `<save_path>/mesh_0.ply`.  Returns (vertices, triangles) on the
+    device.  Decimation (decimate_mesh) stays the caller's step; the outer-region meshes of an unbounded scene come from
+    `export_outer_meshes`."""
     vol = trainer.density_volume(resolution=resolution, density_thresh=density_thresh)
     mean = getattr(trainer, "mean_density", None)
     thresh = min(float(mean.item()), density_thresh) if mean is not None else density_thresh
     v, f = marching_cubes(vol, thresh)
     v = v / (resolution - 1.0) * 2 - 1                      # renderer.py:531
+    if clean is not None:
+        del vol
+        v, f = clean.visibility(v, f)
+        v, f = clean_mesh(v, f, min_f=clean.min_f, min_d=clean.min_d, repair=True)
     os.makedirs(save_path, exist_ok=True)
     write_ply(os.path.join(save_path, "mesh_0.ply"), v, f)
     return v, f
@@ -161,6 +186,14 @@ def remove_selected_vertices(vertices, triangles, removed):
         raise ValueError("remove_selected_vertices: one flag per vertex")
     vkeep = torch.empty(V, dtype=torch.uint8, device=dev); fkeep = torch.empty(Fn, dtype=torch.uint8, device=dev)
     call("n2m_rsv_count", ptr(removed), V, ptr(triangles), Fn, ptr(vkeep), ptr(fkeep), stream())
+    return _emit(vertices, triangles, vkeep, fkeep)
+
+
+def _emit(vertices, triangles, vkeep, fkeep):
+    """the flagged vertices in order and the flagged faces re-indexed (every corner of a flagged face must be flagged): exclusive prefix
+    sums of the flags, one read-back of the output sizes, n2m_rsv_emit"""
+    dev = vertices.device
+    V, Fn = int(vertices.shape[0]), int(triangles.shape[0])
     vinc = torch.cumsum(vkeep, 0, dtype=torch.int32); finc = torch.cumsum(fkeep, 0, dtype=torch.int32)
     nv = int(vinc[-1].item()) if V else 0
     nf = int(finc[-1].item()) if Fn else 0                                   # the host read-backs (output sizes)
@@ -171,14 +204,169 @@ def remove_selected_vertices(vertices, triangles, removed):
     return out_v, out_f
 
 
+# ---- mesh clean-up (csrc/meshclean.cu) -----------------------------------------------------------------------------------------------
+def _pow2(n):
+    return 1 << max(int(n) - 1, 1).bit_length()
+
+
+def _mesh_args(name, vertices, triangles):
+    if not (torch.is_tensor(vertices) and torch.is_tensor(triangles) and vertices.is_cuda and triangles.is_cuda):
+        raise RuntimeError(f"{name}: vertices and triangles must be CUDA tensors (nerf2mesh_b200 has no CPU path)")
+    if vertices.dim() != 2 or vertices.shape[1] != 3 or triangles.dim() != 2 or triangles.shape[1] != 3:
+        raise ValueError(f"{name}: vertices [V,3] and triangles [F,3]")
+    if 3 * triangles.shape[0] >= 2 ** 31 or vertices.shape[0] >= 2 ** 31:
+        raise ValueError(f"{name}: at most 2^31 / 3 faces and 2^31 vertices")
+    if triangles.shape[0] > 0 and vertices.shape[0] == 0:
+        raise ValueError(f"{name}: faces without vertices")
+    return vertices.float().contiguous(), triangles.to(vertices.device, torch.int32).contiguous()
+
+
+def _empty(vertices):
+    return vertices.new_empty(0, 3), torch.empty(0, 3, dtype=torch.int32, device=vertices.device)
+
+
+def _referenced(tri, fkeep, V):
+    vflag = torch.zeros(V, dtype=torch.uint8, device=tri.device)
+    call("n2m_clean_mark_verts", ptr(tri), int(tri.shape[0]), ptr(fkeep), ptr(vflag), stream())
+    return vflag
+
+
 @torch.no_grad()
-def export_outer_meshes(trainer, save_path, env_reso=256, density_thresh=10.0):
-    """export_stage0's outer meshes (non-SDF, renderer.py:606-672) up to their CPU post-processing, for every cascade cas = 1 .. C-1:
+def remove_masked_faces(vertices, triangles, mask, dilation):
+    """remove_masked_trigs (meshutils.py:63-93) on the device.  vertices [V,3] float32, triangles [F,3] int32, mask [F] (0 keeps the face,
+    1 removes it), CUDA.  The faces with mask == 0 are the kept set; each of the `dilation` steps selects every vertex of a kept face and
+    keeps every face with a selected vertex (MeshLab's selection dilation); the other faces and the vertices no kept face references go.
+    Survivors keep their order."""
+    v, tri = _mesh_args("remove_masked_faces", vertices, triangles)
+    V, Fn = int(v.shape[0]), int(tri.shape[0])
+    mask = torch.as_tensor(mask).to(v.device).reshape(-1)
+    if mask.numel() != Fn:
+        raise ValueError("remove_masked_faces: one mask entry per face")
+    if Fn == 0:
+        return _empty(v)
+    fkeep = (mask == 0).to(torch.uint8)
+    vsel = torch.zeros(V, dtype=torch.uint8, device=v.device)
+    for _ in range(int(dilation)):
+        call("n2m_clean_dilate", ptr(tri), Fn, ptr(fkeep), ptr(vsel), stream())
+    return _emit(v, tri, _referenced(tri, fkeep, V), fkeep)
+
+
+@torch.no_grad()
+def clean_mesh(vertices, triangles, v_pct=1, min_f=8, min_d=5, repair=True, info=None):
+    """clean_mesh(..., remesh=False) (meshutils.py:146-188) on the device.  vertices [V,3] float32, triangles [F,3] int32 (CUDA, every index
+    in 0..V-1) -> (vertices, triangles) of the same types.  In order:
+
+    1. vertices no face references go;
+    2. v_pct > 0: close vertices merge with radius r = v_pct / 100 * diag / 10 (diag: the bounding-box diagonal, float64) -- greedily
+       in index order, vertex i leads unless a leader j < i lies within r (float64 dx*dx + dy*dy + dz*dz <= r*r), a non-leader takes the
+       lowest such leader's index; faces that then repeat an index go;
+    3. duplicate faces (the same unordered vertex triple, any winding) go but the lowest;
+    4. faces whose float64 cross(b - a, c - a) is the zero vector go;
+    5. min_d > 0: edge-connected components (faces sharing two vertices) whose bounding-box diagonal is < min_d / 100 * diag go (diag of
+       the vertices still referenced);
+    6. min_f > 0: components of fewer than min_f faces go;
+    7. repair: the faces on an edge of more than two faces are visited by ascending float64 area (then index); a face goes when one of
+       its edges still has more than two faces;
+    8. repair: a vertex whose faces form k > 1 fans (faces joined through an edge at the vertex) is split: the fan with the lowest face
+       keeps it, each other fan gets a copy appended after all vertices, in (vertex, lowest face of the fan) order.
+
+    Surviving vertices and faces keep their order; the vertices no face references at the end go.  The percentage readings of steps 2
+    and 5 are this library's (pymeshlab is not run to confirm them).  `info`, a dict, receives `merge_rounds`: the decision rounds of
+    step 2, each one launch and one read-back of a flag."""
+    v, tri = _mesh_args("clean_mesh", vertices, triangles)
+    tri = tri.clone()                                                        # re-indexed in place by the merge and the split
+    dev = v.device
+    V, Fn = int(v.shape[0]), int(tri.shape[0])
+    rounds = 0
+    if info is not None:
+        info["merge_rounds"] = 0
+    if Fn == 0:
+        return _empty(v)
+    i32 = dict(dtype=torch.int32, device=dev)
+    fkeep = torch.ones(Fn, dtype=torch.uint8, device=dev)
+    bbox = torch.empty(6, **i32)
+    if v_pct > 0:                                                            # 1. + 2.
+        vflag = _referenced(tri, None, V)
+        call("n2m_clean_bbox", ptr(v), V, ptr(vflag), ptr(bbox), stream())
+        nb = _pow2(2 * V)
+        count = torch.zeros(nb, **i32); vbucket = torch.empty(V, **i32)
+        call("n2m_clean_merge_bin", ptr(v), V, ptr(vflag), ptr(bbox), float(v_pct), nb, ptr(count), ptr(vbucket), stream())
+        start = torch.zeros(nb + 1, **i32)
+        torch.cumsum(count, 0, dtype=torch.int32, out=start[1:])
+        cursor = start[:-1].clone(); items = torch.empty(V, **i32)
+        call("n2m_clean_merge_fill", V, ptr(vflag), ptr(vbucket), ptr(cursor), ptr(items), stream())
+        decided = torch.zeros(V, **i32); target = torch.empty(V, **i32); pending = torch.zeros(1, **i32)
+        while True:
+            rounds += 1
+            pending.zero_()
+            call("n2m_clean_merge_round", ptr(v), V, ptr(vflag), ptr(bbox), float(v_pct), nb, ptr(start), ptr(items), rounds, ptr(decided),
+                 ptr(target), ptr(pending), stream())
+            if not int(pending.item()):                                      # the round-termination read-back
+                break
+        del count, vbucket, start, cursor, items, decided
+        call("n2m_clean_merge_apply", ptr(tri), Fn, ptr(target), ptr(fkeep), stream())
+        if info is not None:
+            info["merge_rounds"] = rounds
+    nt = _pow2(2 * Fn)                                                       # 3. + 4.
+    table, slot_of = torch.empty(nt, **i32), torch.empty(Fn, **i32)
+    call("n2m_clean_dup_null", ptr(v), ptr(tri), Fn, ptr(fkeep), nt, ptr(table), ptr(slot_of), stream())
+    if min_d > 0 or min_f > 0 or repair:
+        ne = _pow2(6 * Fn)
+        table = torch.empty(ne, **i32); slot_of = torch.empty(3 * Fn, **i32)
+        call("n2m_clean_edge_table", ptr(tri), Fn, ptr(fkeep), ne, ptr(table), ptr(slot_of), stream())
+    if min_d > 0 or min_f > 0:                                               # 5. + 6.
+        vflag = _referenced(tri, fkeep, V)
+        call("n2m_clean_bbox", ptr(v), V, ptr(vflag), ptr(bbox), stream())
+        parent, label, count = (torch.empty(Fn, **i32) for _ in range(3))
+        cmin, cmax = torch.empty(3 * Fn, **i32), torch.empty(3 * Fn, **i32)
+        call("n2m_clean_components", ptr(v), ptr(tri), Fn, ptr(fkeep), ptr(table), ptr(slot_of), ptr(bbox), float(max(min_d, 0)),
+             int(max(min_f, 0)), ptr(parent), ptr(label), ptr(count), ptr(cmin), ptr(cmax), stream())
+        del parent, label, count, cmin, cmax
+    if repair:                                                               # 7. + 8.
+        # once slot_of is known the table's slots are free: they hold the per-edge live face counts, then the per-edge lowest face-edge
+        cap = _pow2(3 * Fn)
+        keys, vals, ncand = torch.empty(cap, dtype=torch.int64, device=dev), torch.empty(cap, **i32), torch.empty(1, **i32)
+        call("n2m_clean_nm_edges", ptr(v), ptr(tri), Fn, ptr(fkeep), ptr(slot_of), ne, ptr(table), ptr(ncand), ptr(keys), ptr(vals), cap,
+             stream())
+        cparent, clabel, cnew = (torch.empty(3 * Fn, **i32) for _ in range(3))
+        vmin, nextra = torch.empty(V, **i32), torch.empty(1, **i32)
+        call("n2m_clean_nm_verts_find", ptr(tri), V, Fn, ptr(fkeep), ptr(slot_of), ne, ptr(table), ptr(cparent), ptr(clabel), ptr(vmin),
+             ptr(nextra), ptr(keys), ptr(vals), ptr(cnew), cap, stream())
+        n = int(nextra.item())                                               # read-back: the number of vertex copies (output size)
+        ext = torch.empty(V + n, 3, device=dev)
+        ext[:V] = v
+        call("n2m_clean_nm_verts_apply", ptr(v), V, ptr(tri), Fn, ptr(fkeep), ptr(clabel), ptr(vmin), ptr(cnew), ptr(ext), stream())
+        v, V = ext, V + n
+    return _emit(v, tri, _referenced(tri, fkeep, V), fkeep)
+
+
+class CleanOptions:
+    """the reference's post-processing of the stage-0 meshes (`clean=` of export_stage0_mesh / export_outer_meshes): clean_mesh with
+    min_f / min_d (opt.clean_min_f, opt.clean_min_d), and -- when mvps, H, W are given (the `mesh_visibility_culling` of -O) -- the faces
+    no view sees removed with remove_masked_faces(dilation=visibility_mask_dilation)"""
+
+    def __init__(self, min_f=8, min_d=5, visibility_mask_dilation=5, mvps=None, H=None, W=None):
+        if mvps is not None and (H is None or W is None):
+            raise ValueError("CleanOptions: the visibility test needs mvps, H and W")
+        self.min_f, self.min_d, self.visibility_mask_dilation = min_f, min_d, visibility_mask_dilation
+        self.mvps, self.H, self.W = mvps, H, W
+
+    def visibility(self, v, f):
+        """remove_masked_faces over mark_unseen_triangles, or the mesh unchanged without views"""
+        if self.mvps is None or f.shape[0] == 0:
+            return v, f
+        return remove_masked_faces(v, f, mark_unseen_triangles(v, f, self.mvps, self.H, self.W), self.visibility_mask_dilation)
+
+
+@torch.no_grad()
+def export_outer_meshes(trainer, save_path, env_reso=256, density_thresh=10.0, *, clean=None):
+    """export_stage0's outer meshes (non-SDF, renderer.py:606-672) up to their decimation, for every cascade cas = 1 .. C-1:
     occupancy volume of density_grid[cas] at env_reso^3 -> marching cubes at 0.5 -> (idx / (R-1) * 2 - 1) * (bound - half) with
     bound = min(2^cas, cfg.bound), half = bound / R -> removal of the centre box and of the region outside the trainer's AABB shrunk by
-    half -> `<save_path>/mesh_{cas}.ply`.  Returns {cas: (vertices [V,3] float32, triangles [F,3] int32)} on the device; a cascade left
-    without vertices writes no file and is not in the dict.  The caller's CPU code then cleans and decimates each mesh (clean_mesh,
-    decimate_mesh with decimate_target // 2) and may drop the faces no training view sees (mark_unseen_triangles + remove_masked_trigs)."""
+    half -> with `clean` (a CleanOptions): clean_mesh(repair=False), then the visibility test and remove_masked_faces when it carries
+    views (:651-668) -> `<save_path>/mesh_{cas}.ply`.  Returns {cas: (vertices [V,3] float32, triangles [F,3] int32)} on the device; a
+    cascade left without vertices writes no file and is not in the dict.  Decimation (decimate_mesh with decimate_target // 2, between the
+    clean-up and the visibility test in the reference) stays the caller's step."""
     if hasattr(trainer, "drop_prefetch"):
         trainer.drop_prefetch()
     c = trainer.cfg
@@ -197,6 +385,10 @@ def export_outer_meshes(trainer, save_path, env_reso=256, density_thresh=10.0):
             continue
         v, removed = outer_select(v, R, bound - half, (xmn + half, ymn + half, zmn + half, xmx - half, ymx - half, zmx - half))
         v, f = remove_selected_vertices(v, f, removed)
+        if clean is not None:
+            v, f = clean_mesh(v, f, min_f=clean.min_f, min_d=clean.min_d, repair=False)
+            if v.shape[0] > 0:
+                v, f = clean.visibility(v, f)
         if v.shape[0] == 0:
             continue
         write_ply(os.path.join(save_path, f"mesh_{cas}.ply"), v, f)

@@ -3,8 +3,8 @@
  * NeRFRenderer.export_stage0 (nerf/renderer.py:471-545) evaluates the density on a regular grid, copies it to the host and calls the
  * third-party PyMCubes `mcubes.marching_cubes(sigmas, density_thresh)` (:526-529; not vendored, version unpinned) before cleaning /
  * decimating the mesh with CPU mesh libraries.  These entry points replace the marching-cubes call on the device; the volume comes from
- * Stage0Trainer.density_volume (the reference's own arithmetic up to that call, tests/test_gpu_reference_parity.py), the cleaning /
- * decimation stays the reference's CPU code.  Python binding: nerf2mesh_b200/mesh.py (`marching_cubes(volume, isovalue)` returns
+ * Stage0Trainer.density_volume (the reference's own arithmetic up to that call, tests/test_gpu_reference_parity.py); the cleaning and
+ * the decimation that follow run on the device too (below).  Python binding: nerf2mesh_b200/mesh.py (`marching_cubes(volume, isovalue)` returns
  * vertices in index coordinates and int32 triangles like PyMCubes).
  *
  *   n2m_mc_count : volume [X,Y,Z] f32 (z fastest), per grid point: vcount = iso-crossings on its +x / +y / +z edges, tcount = triangles
@@ -59,6 +59,32 @@
  *                             corner's fan root) and vmin feed n2m_clean_nm_verts_apply
  *   n2m_clean_nm_verts_apply: the corners of those fans take vertex V + cnew, ext_vertices [V + nextra, 3] f32 rows V.. get the copies'
  *                             positions (the caller copies rows 0..V-1)
+ *
+ * Decimation (meshing_decimation_quadric_edge_collapse of meshutils.py decimate_mesh, pymeshlab in the reference; csrc/decimate.cu;
+ * Python: mesh.decimate_mesh).  Rounds of independent edge collapses over fkeep / tri as above: each round rebuilds the edge table
+ * (n2m_clean_edge_table) and the vertex -> live face lists, keys every valid collapse, selects, moves the survivors and re-indexes the
+ * faces with n2m_clean_merge_apply; the caller reads flive once per round and compacts once with n2m_rsv_emit.  The lower vertex of a
+ * collapsed edge survives.  Q [V,10] f64 holds a00 a01 a02 a11 a12 a22 b0 b1 b2 c of each vertex quadric.
+ *   n2m_decim_init      : fkeep [F] u8 = the face repeats no index; flive [1] i32 = the number of such faces (initialised here)
+ *   n2m_decim_vcount    : vcount [V] i32 += the live faces at each vertex (caller zeroes)
+ *   n2m_decim_vfill     : cursor = EXCLUSIVE prefix sum of vcount (advanced here) -> vfaces [3 * live] i32, each vertex's live faces in
+ *                         any order
+ *   n2m_decim_quadrics  : Q [V,10] = the sum over the vertex's live faces, in ascending face index from +0, of the plane quadric of the
+ *                         float64 unit normal u = cross(b - a, c - a) / |.| and d = -u.a (zero for |cross| = 0); sorts each list of vfaces
+ *   n2m_decim_edges     : ecount [nslots] i32 = live face-edges per slot of n2m_clean_edge_table's slot_of; vbnd [V] u8 = the vertex is
+ *                         on an edge of one live face (both initialised here)
+ *   n2m_decim_eval      : keys [3F] u64, pos [3F,3] f32: for the lowest live face-edge e of an edge (a < b) whose collapse is valid,
+ *                         pos[e] = the merged position and keys[e] = fkey(float(cost)) << 32 | e, else keys[e] = ~0.  Valid: 1 or 2
+ *                         faces; every common neighbour of a and b is an opposite vertex; a boundary edge or not both ends boundary; a
+ *                         boundary edge's face has not both other edges on the boundary; not (a,c,d) and (b,c,d) both live; no other
+ *                         face at a or b gets float64 dot(n_old, n_new) <= 0.  Position (optimal
+ *                         != 0): A p = -b of Q_a + Q_b by cofactors when det > 1e-6 trace^3, else the cheapest of a, b, the midpoint
+ *                         (ties in that order); optimal == 0: the float64 midpoint; rounded once to f32, cost = the quadric there
+ *   n2m_decim_threshold : state [4] u64, state[3] = K*: the least key at which the valid keys in order, weighted by their edge's face
+ *                         count, reach flive - target (every valid key when they do not); hist [256] u64 and state[0..2] are scratch
+ *   n2m_decim_select    : the valid edges with key <= K* equal to the least such key over the closed neighbourhoods of both ends:
+ *                         target [V] i32 = b -> a (identity elsewhere), vertices[a] = pos, Q[a] += Q[b], flive -= the edge's faces;
+ *                         vmin, r1 [V] u64 are scratch.  The caller then runs n2m_clean_merge_apply with target
  */
 #ifndef N2M_B200_MESH_H
 #define N2M_B200_MESH_H
@@ -106,6 +132,22 @@ int n2m_clean_nm_verts_find(const int32_t* tri, uint32_t V, uint32_t F, const ui
                             int32_t* cnew, uint32_t capacity, n2m_stream_t stream);
 int n2m_clean_nm_verts_apply(const float* vertices, uint32_t V, int32_t* tri, uint32_t F, const uint8_t* fkeep, const int32_t* clabel,
                              const int32_t* vmin, const int32_t* cnew, float* ext_vertices, n2m_stream_t stream);
+
+int n2m_decim_init(const int32_t* tri, uint32_t F, uint8_t* fkeep, int32_t* flive, n2m_stream_t stream);
+int n2m_decim_vcount(const int32_t* tri, uint32_t F, const uint8_t* fkeep, int32_t* vcount, n2m_stream_t stream);
+int n2m_decim_vfill(const int32_t* tri, uint32_t F, const uint8_t* fkeep, int32_t* cursor, int32_t* vfaces, n2m_stream_t stream);
+int n2m_decim_quadrics(const float* vertices, uint32_t V, const int32_t* tri, const int32_t* vstart, int32_t* vfaces, double* Q,
+                       n2m_stream_t stream);
+int n2m_decim_edges(const int32_t* tri, uint32_t V, uint32_t F, const uint8_t* fkeep, const int32_t* slot_of, uint32_t nslots, int32_t* ecount,
+                    uint8_t* vbnd, n2m_stream_t stream);
+int n2m_decim_eval(const float* vertices, const double* Q, const int32_t* tri, uint32_t F, const uint8_t* fkeep, const int32_t* table,
+                   const int32_t* slot_of, const int32_t* ecount, const uint8_t* vbnd, const int32_t* vstart, const int32_t* vfaces, int optimal,
+                   uint64_t* keys, float* pos, n2m_stream_t stream);
+int n2m_decim_threshold(const uint64_t* keys, uint32_t F, const int32_t* slot_of, const int32_t* ecount, const int32_t* flive, uint32_t target,
+                        uint64_t* hist, uint64_t* state, n2m_stream_t stream);
+int n2m_decim_select(const uint64_t* keys, uint32_t V, uint32_t F, const int32_t* tri, const int32_t* slot_of, const int32_t* ecount,
+                     const int32_t* vstart, const int32_t* vfaces, const uint64_t* state, const float* pos, uint64_t* vmin, uint64_t* r1,
+                     float* vertices, double* Q, int32_t* target, int32_t* flive, n2m_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -20,6 +20,7 @@
 //   k_nme_*                         non-manifold edges: the faces on an edge of > 2 live faces, visited by (float64 area, index) in one CTA
 //   k_fan_*                         non-manifold vertices: union-find over face corners joined through an edge at their vertex
 #include "n2m_common.cuh"
+#include "mesh_keys.cuh"
 #include "../../include/n2m_b200_mesh.h"
 
 #include <limits.h>
@@ -29,12 +30,7 @@ namespace {
 
 constexpr int kSortThreads = 1024;
 
-// ---- float keys and the two percentage readings ---------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t fkey(float x) {
-    const uint32_t u = __float_as_uint(x);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float fkey_inv(uint32_t k) { return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k); }
+// ---- the two percentage readings --------------------------------------------------------------------------------------------------
 
 // sqrt((dx*dx + dy*dy) + dz*dz) of a key box, each operation rounded on its own; an empty box (min > max) has diagonal 0
 __device__ double box_diag(const uint32_t* lo, const uint32_t* hi) {

@@ -6,20 +6,23 @@ third-party CPU library) with the kernels of csrc/mcubes.cu (C ABI include/n2m_b
     vertices, triangles = marching_cubes(volume, isovalue)      # volume [X,Y,Z] float32 CUDA tensor
     # vertices [V,3] float32 in index coordinates (0 .. X-1), triangles [F,3] int32 -- the form PyMCubes returns (as tensors)
 
-`export_stage0_mesh(trainer, path, resolution)` is the reference's export up to (not including) its decimation: density volume
-(Stage0Trainer.density_volume == renderer.py:480-524) -> marching cubes -> `vertices / (resolution - 1) * 2 - 1` (:531) -> with
-`clean=CleanOptions(...)` the visibility test, remove_masked_faces and clean_mesh -> `mesh_0.ply`.  No CPU fallback: the volume must
+`export_stage0_mesh(trainer, path, resolution)` is the reference's export: density volume (Stage0Trainer.density_volume ==
+renderer.py:480-524) -> marching cubes -> `vertices / (resolution - 1) * 2 - 1` (:531) -> with `clean=CleanOptions(...)` the visibility
+test, remove_masked_faces and clean_mesh -> with `decimate_target=` decimate_mesh -> `mesh_0.ply`.  No CPU fallback: the volume must
 live on a CUDA device.
 
 The reference's pymeshlab post-processing (meshutils.py) is restated as exact rules in csrc/meshclean.cu: `remove_masked_faces`
 (remove_masked_trigs: the faces a mask keeps, dilated along shared vertices) and `clean_mesh` (clean_mesh(..., remesh=False): close-vertex
-merge, duplicate and null faces, small components, non-manifold edges and vertices).  The mesh stays on the device from marching cubes to
-the PLY writer; the host reads back output sizes and the merge's round flags only.  Decimation (decimate_mesh) is not here.
+merge, duplicate and null faces, small components, non-manifold edges and vertices).  `decimate_mesh` (csrc/decimate.cu) restates
+meshing_decimation_quadric_edge_collapse as rounds of independent quadric edge collapses, this library's own deterministic rule.  The mesh
+stays on the device from marching cubes to the PLY writer; the host reads back output sizes, the merge's round flags and one face count
+per decimation round only.
 
 Unbounded scenes (bound > 1, C = 1 + ceil(log2(bound)) cascades) also get one mesh per outer cascade (csrc/cascade.cu):
-`export_outer_meshes(trainer, path, env_reso)` is the non-SDF branch of export_stage0 for cas = 1 .. C-1 (renderer.py:606-672) up to its
-decimation -- occupancy volume of density_grid[cas] -> marching cubes at 0.5 -> world coordinates (float64, rounded once) -> removal of
-the centre box and of what lies outside the training AABB -> with `clean=` clean_mesh and the visibility test -> `mesh_{cas}.ply`.
+`export_outer_meshes(trainer, path, env_reso)` is the non-SDF branch of export_stage0 for cas = 1 .. C-1 (renderer.py:606-672) --
+occupancy volume of density_grid[cas] -> marching cubes at 0.5 -> world coordinates (float64, rounded once) -> removal of the centre box
+and of what lies outside the training AABB -> with `clean=` clean_mesh -> with `decimate_target=` decimate_mesh to half of it -> with
+`clean=` the visibility test -> `mesh_{cas}.ply`.
 `mark_unseen_triangles` is the reference's visibility test on those meshes, `load_stage0_meshes` picks every cascade's mesh up again for
 stage 1.
 """
@@ -58,6 +61,14 @@ _lib.register({
     "n2m_clean_nm_edges": [P, P, U, P, P, U, P, P, P, P, U, P],
     "n2m_clean_nm_verts_find": [P, U, U, P, P, U, P, P, P, P, P, P, P, P, U, P],
     "n2m_clean_nm_verts_apply": [P, U, P, U, P, P, P, P, P, P],
+    "n2m_decim_init": [P, U, P, P, P],
+    "n2m_decim_vcount": [P, U, P, P, P],
+    "n2m_decim_vfill": [P, U, P, P, P, P],
+    "n2m_decim_quadrics": [P, U, P, P, P, P, P],
+    "n2m_decim_edges": [P, U, U, P, P, U, P, P, P],
+    "n2m_decim_eval": [P, P, P, U, P, P, P, P, P, P, P, ctypes.c_int, P, P, P],
+    "n2m_decim_threshold": [P, U, P, P, P, U, P, P, P],
+    "n2m_decim_select": [P, U, U, P, P, P, P, P, P, P, P, P, P, P, P, P, P],
 })
 
 _tables = {}
@@ -123,12 +134,12 @@ def read_ply(path):
     return v.copy(), faces["i"].copy()
 
 
-def export_stage0_mesh(trainer, save_path, resolution=512, density_thresh=10.0, *, clean=None):
-    """NeRFRenderer.export_stage0 for the inner region up to its decimation (renderer.py:471-544): density volume -> marching cubes at
+def export_stage0_mesh(trainer, save_path, resolution=512, density_thresh=10.0, *, clean=None, decimate_target=0):
+    """NeRFRenderer.export_stage0 for the inner region (renderer.py:471-544): density volume -> marching cubes at
     min(mean_density, density_thresh) -> world coordinates -> with `clean` (a CleanOptions): the visibility test and remove_masked_faces
-    when it carries views, then clean_mesh(repair=True) (:531-537) -> `<save_path>/mesh_0.ply`.  Returns (vertices, triangles) on the
-    device.  Decimation (decimate_mesh) stays the caller's step; the outer-region meshes of an unbounded scene come from
-    `export_outer_meshes`."""
+    when it carries views, then clean_mesh(repair=True) (:531-537) -> with decimate_target > 0 and more faces than int(decimate_target):
+    decimate_mesh to that many faces with optimal placement (:540-541) -> `<save_path>/mesh_0.ply`.  Returns (vertices, triangles) on the
+    device.  The outer-region meshes of an unbounded scene come from `export_outer_meshes`."""
     vol = trainer.density_volume(resolution=resolution, density_thresh=density_thresh)
     mean = getattr(trainer, "mean_density", None)
     thresh = min(float(mean.item()), density_thresh) if mean is not None else density_thresh
@@ -138,6 +149,8 @@ def export_stage0_mesh(trainer, save_path, resolution=512, density_thresh=10.0, 
         del vol
         v, f = clean.visibility(v, f)
         v, f = clean_mesh(v, f, min_f=clean.min_f, min_d=clean.min_d, repair=True)
+    if decimate_target > 0 and f.shape[0] > int(decimate_target):
+        v, f = decimate_mesh(v, f, int(decimate_target), optimal_placement=True)
     os.makedirs(save_path, exist_ok=True)
     write_ply(os.path.join(save_path, "mesh_0.ply"), v, f)
     return v, f
@@ -358,15 +371,102 @@ class CleanOptions:
         return remove_masked_faces(v, f, mark_unseen_triangles(v, f, self.mvps, self.H, self.W), self.visibility_mask_dilation)
 
 
+# ---- decimation (csrc/decimate.cu) ---------------------------------------------------------------------------------------------------
 @torch.no_grad()
-def export_outer_meshes(trainer, save_path, env_reso=256, density_thresh=10.0, *, clean=None):
-    """export_stage0's outer meshes (non-SDF, renderer.py:606-672) up to their decimation, for every cascade cas = 1 .. C-1:
-    occupancy volume of density_grid[cas] at env_reso^3 -> marching cubes at 0.5 -> (idx / (R-1) * 2 - 1) * (bound - half) with
-    bound = min(2^cas, cfg.bound), half = bound / R -> removal of the centre box and of the region outside the trainer's AABB shrunk by
-    half -> with `clean` (a CleanOptions): clean_mesh(repair=False), then the visibility test and remove_masked_faces when it carries
-    views (:651-668) -> `<save_path>/mesh_{cas}.ply`.  Returns {cas: (vertices [V,3] float32, triangles [F,3] int32)} on the device; a
-    cascade left without vertices writes no file and is not in the dict.  Decimation (decimate_mesh with decimate_target // 2, between the
-    clean-up and the visibility test in the reference) stays the caller's step."""
+def decimate_mesh(vertices, triangles, target, optimal_placement=True, info=None):
+    """Quadric edge-collapse decimation to `target` faces on the device: the library's parallel reading of pymeshlab's
+    meshing_decimation_quadric_edge_collapse (meshutils.py decimate_mesh, VCG) with its defaults.  vertices [V,3] float32, triangles [F,3]
+    int32 (CUDA) -> (vertices, triangles) of the same types.  ValueError when target < 1.  F <= target: no collapse, only the vertices no
+    face references go.
+
+    Otherwise faces that repeat an index go, and rounds of collapses run while more than `target` faces live:
+    - quadrics: each face's plane quadric from its float64 unit normal n = cross(b - a, c - a) / |.| and d = -n.a, without area weight
+      (zero when |cross| = 0); a vertex sums those of its faces in ascending face index;
+    - placement of the merged vertex of edge (a, b), a < b, with Q = Q_a + Q_b: optimal_placement solves A p = -b when
+      det(A) > 1e-6 trace(A)^3 (every eigenvalue above 1e-6 of the trace), else takes the cheapest of a, b and the midpoint (ties in that
+      order); without it, the float64 midpoint.  The position is rounded once to float32; the cost is Q at that point;
+    - validity: the edge has 1 or 2 live faces; every vertex adjacent to both a and b is an opposite vertex of those faces (link
+      condition); it is a boundary edge or not both ends are boundary vertices; a boundary edge's face does not have its other two edges
+      on the boundary too (a lone triangle would vanish, and with it a component); not both (a, c, d) and (b, c, d) are live faces for
+      its opposite vertices c, d; and no other face at a or b flips or degenerates (float64 dot(n_old, n_new) <= 0).  A manifold mesh
+      stays manifold and keeps its Euler characteristic;
+    - key: fkey(float32(cost)) << 32 | e, e the edge's lowest live face-edge 3f + k (faces keep their input index between rounds);
+    - budget: K* is the least key at which the valid edges in key order, each counted with its 1 or 2 faces, remove at least
+      (live faces - target); only keys <= K* may be selected, so the last round ends at target or target - 1 faces;
+    - selection: vmin[v] = the least such key at v, r1[v] = the least vmin over v and its neighbours; an edge whose key equals r1 at
+      both ends is selected.  Selected edges share no vertex and no adjacency, so the round equals their collapses in any order;
+    - apply: a survives at the float32 position with Q_a + Q_b, every face re-indexes b -> a, and the faces that then repeat an index go.
+    The rounds stop at <= target faces or when a round selects nothing (stalled).  Surviving vertices and faces keep their order, and the
+    vertices no face references go (VCG's autoclean).
+
+    VCG collapses one edge at a time from a heap, with a quality-threshold penalty and its own placement; this rule keeps its defaults'
+    reading (preserveboundary=False, preservetopology=False, planarquadric=False, autoclean=True, no quality penalty) and is not claimed
+    to reproduce its output.  `info`, a dict, receives `rounds` (rounds that collapsed something), `stalled` and `faces` (live faces after
+    each round); the host reads back one count per round and the output sizes."""
+    v, tri = _mesh_args("decimate_mesh", vertices, triangles)
+    target = int(target)
+    if target < 1:
+        raise ValueError("decimate_mesh: target must be at least 1")
+    dev = v.device
+    V, Fn = int(v.shape[0]), int(tri.shape[0])
+    rounds, faces, stalled = 0, [], False
+    if Fn == 0:
+        out = _empty(v)
+    elif Fn <= target:
+        out = _emit(v, tri, _referenced(tri, None, V), torch.ones(Fn, dtype=torch.uint8, device=dev))
+    else:
+        v, tri = v.clone(), tri.clone()                                      # positions move and faces re-index in place
+        i32, i64 = dict(dtype=torch.int32, device=dev), dict(dtype=torch.int64, device=dev)
+        fkeep, flive = torch.empty(Fn, dtype=torch.uint8, device=dev), torch.empty(1, **i32)
+        call("n2m_decim_init", ptr(tri), Fn, ptr(fkeep), ptr(flive), stream())
+        ne = _pow2(6 * Fn)
+        table, ecount, slot_of = torch.empty(ne, **i32), torch.empty(ne, **i32), torch.empty(3 * Fn, **i32)
+        vcount, vstart, vfaces = torch.empty(V, **i32), torch.zeros(V + 1, **i32), torch.empty(3 * Fn, **i32)
+        vbnd = torch.empty(V, dtype=torch.uint8, device=dev)
+        keys, pos = torch.empty(3 * Fn, **i64), torch.empty(3 * Fn, 3, device=dev)
+        Q = torch.empty(V, 10, dtype=torch.float64, device=dev)
+        hist, state, vmin, r1 = torch.empty(256, **i64), torch.empty(4, **i64), torch.empty(V, **i64), torch.empty(V, **i64)
+        vtarget = torch.empty(V, **i32)
+        live = int(flive.item())                                             # read-back: live faces
+        while live > target:
+            call("n2m_clean_edge_table", ptr(tri), Fn, ptr(fkeep), ne, ptr(table), ptr(slot_of), stream())
+            vcount.zero_()
+            call("n2m_decim_vcount", ptr(tri), Fn, ptr(fkeep), ptr(vcount), stream())
+            torch.cumsum(vcount, 0, dtype=torch.int32, out=vstart[1:])
+            cursor = vstart[:-1].clone()
+            call("n2m_decim_vfill", ptr(tri), Fn, ptr(fkeep), ptr(cursor), ptr(vfaces), stream())
+            if rounds == 0:
+                call("n2m_decim_quadrics", ptr(v), V, ptr(tri), ptr(vstart), ptr(vfaces), ptr(Q), stream())
+            call("n2m_decim_edges", ptr(tri), V, Fn, ptr(fkeep), ptr(slot_of), ne, ptr(ecount), ptr(vbnd), stream())
+            call("n2m_decim_eval", ptr(v), ptr(Q), ptr(tri), Fn, ptr(fkeep), ptr(table), ptr(slot_of), ptr(ecount), ptr(vbnd), ptr(vstart),
+                 ptr(vfaces), int(bool(optimal_placement)), ptr(keys), ptr(pos), stream())
+            call("n2m_decim_threshold", ptr(keys), Fn, ptr(slot_of), ptr(ecount), ptr(flive), target, ptr(hist), ptr(state), stream())
+            call("n2m_decim_select", ptr(keys), V, Fn, ptr(tri), ptr(slot_of), ptr(ecount), ptr(vstart), ptr(vfaces), ptr(state), ptr(pos),
+                 ptr(vmin), ptr(r1), ptr(v), ptr(Q), ptr(vtarget), ptr(flive), stream())
+            call("n2m_clean_merge_apply", ptr(tri), Fn, ptr(vtarget), ptr(fkeep), stream())
+            now = int(flive.item())                                          # the round's read-back: live faces
+            if now == live:
+                stalled = True
+                break
+            rounds += 1
+            faces.append(now)
+            live = now
+        del table, ecount, slot_of, vcount, vstart, vfaces, vbnd, keys, pos, Q, vmin, r1, vtarget
+        out = _emit(v, tri, _referenced(tri, fkeep, V), fkeep)
+    if info is not None:
+        info.update(rounds=rounds, stalled=stalled, faces=faces)
+    return out
+
+
+@torch.no_grad()
+def export_outer_meshes(trainer, save_path, env_reso=256, density_thresh=10.0, *, clean=None, decimate_target=0):
+    """export_stage0's outer meshes (non-SDF, renderer.py:606-672), for every cascade cas = 1 .. C-1: occupancy volume of
+    density_grid[cas] at env_reso^3 -> marching cubes at 0.5 -> (idx / (R-1) * 2 - 1) * (bound - half) with bound = min(2^cas, cfg.bound),
+    half = bound / R -> removal of the centre box and of the region outside the trainer's AABB shrunk by half -> with `clean` (a
+    CleanOptions): clean_mesh(repair=False) -> with decimate_target > 0 and more faces than int(decimate_target) // 2: decimate_mesh to
+    that many faces without optimal placement (:609, :657-659) -> with `clean` carrying views: the visibility test and
+    remove_masked_faces (:661-668) -> `<save_path>/mesh_{cas}.ply`.  Returns {cas: (vertices [V,3] float32, triangles [F,3] int32)} on
+    the device; a cascade left without vertices writes no file and is not in the dict."""
     if hasattr(trainer, "drop_prefetch"):
         trainer.drop_prefetch()
     c = trainer.cfg
@@ -387,8 +487,11 @@ def export_outer_meshes(trainer, save_path, env_reso=256, density_thresh=10.0, *
         v, f = remove_selected_vertices(v, f, removed)
         if clean is not None:
             v, f = clean_mesh(v, f, min_f=clean.min_f, min_d=clean.min_d, repair=False)
-            if v.shape[0] > 0:
-                v, f = clean.visibility(v, f)
+        half_target = int(decimate_target) // 2
+        if v.shape[0] > 0 and half_target > 0 and f.shape[0] > half_target:
+            v, f = decimate_mesh(v, f, half_target, optimal_placement=False)
+        if clean is not None and v.shape[0] > 0:
+            v, f = clean.visibility(v, f)
         if v.shape[0] == 0:
             continue
         write_ply(os.path.join(save_path, f"mesh_{cas}.ply"), v, f)

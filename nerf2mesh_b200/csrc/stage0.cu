@@ -249,6 +249,21 @@ k_s0_records(const int32_t* __restrict__ rays, const float2* __restrict__ tbuf, 
 //                 density-grid update (renderer.py:1112-1113 evaluates self.density on cell centres), stage 1 and tests.
 // (The TV gradient is not evaluated here although 4 of its 7 stencil values are in registers: it slows this kernel by more than a
 // separate TV launch costs, and that launch hides under the MLP kernels.)
+//
+// Where the time goes (profiles/gather_time.py, H100 80GB HBM3 at 700 W, bench.py's batches).  Lego (M = 285,107): the whole
+// batch takes 114 us with a warm L2 and 124 us with a cold one, a part 70-72 us warm and 78-84 us cold; garden (M = 823,460):
+// 284 / 294 us.  The batch touches 1.19 M sectors (38 MB) of the table, but its warp loads request 17.3 M sectors (554 MB) from L2,
+// every corner of a hashed level a sector of its own: 4.9 TB/s at 114 us, more than HBM could deliver.  So the table sectors come
+// from L2, and the 10 us between cold and warm is all an L2-resident table could save.  What follows from it, measured the same way:
+//  * A level-group walk like the scatter's, writing each level's three fp16 features to per-level planes (1 KiB per tile and level,
+//    whole sectors) and then building each tile image from its 16 planes in place, gave bit-identical images but 134 us for the
+//    lego batch, 87-103 us per part, a 1.16 ms step timeline instead of 1.03 ms and 7 % fewer samples/s in bench.py.  The walk
+//    leaves the sector requests as they were, already served by L2, and adds a re-read of the records per group and the planes.
+//  * Issuing the 8 loads of level l + 1 before the sums of level l (two levels in flight): 110 us on lego, 250 us on garden, same
+//    bits, but the step is no faster (lego 285.8-286.0 M samples/s against 286.0-288.3, garden 371.2-371.8 against 372.1-373.4).
+//    In the step the gathers share the device with TV (half of it) and with each other: part 0's gather ended 44 us earlier, but its
+//    k_mlp_fwd started 13 us later, queued behind part 1's gather for SM slots, and TV ended 16 us later.
+//  * One 16 B load for the two x-neighbour corners whenever their rows form an aligned pair: 132 us on lego.
 template <bool POINTS>
 __device__ __forceinline__ void
 encode_fwd_tile(const n2m_s0_params& p, const float4* __restrict__ recs,

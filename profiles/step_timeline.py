@@ -36,6 +36,8 @@ TV = "k_s0_encode_bwd<false, true>"
 
 
 def stage(name):
+    if name.startswith("k_s0_composite_loss"):          # k_s0_composite_loss<ADAPTIVE>
+        return "k_s0_composite_loss"
     return "scatter" if name in SCATTERS else name
 
 

@@ -27,7 +27,7 @@
  *              red.global.add.v4.f32 per lattice corner.
  *   enc_tiles  one 16 KiB image per 128 samples: fp16 [128 x 64] in the no-swizzle core-matrix layout
  *              (chunk-major, wg.cuh): cols 0-2 xyz, 3-18 density features, 19-50 colour features,
- *              51-53 unit view direction, 54-63 zero.  It is the A operand of every first-layer GEMM and is
+ *              51-53 unit view direction, 54..53+ind_dim appearance codes, rest zero (see "Per-image appearance codes").  It is the A operand of every first-layer GEMM and is
  *              staged global->shared with a single bulk async copy.
  *   recs       [Mcap] float4 {t_before, dt, t_after, ray_id (bits)} per sample, ray order.
  *   counters   int32 [17]: [0] M (total samples marched), [1] min(M, Mcap), [2] overflow flag, [3] / [15] samples inside / outside the
@@ -76,6 +76,9 @@ typedef struct {
     uint32_t shading_full;  /* 0 = 'diffuse' (first diffuse_step iterations), 1 = 'full'; 2 = 'specular': n2m_s0_mlp_fwd only (evaluation),
                                which then writes (sigma, specular) -- the training and backward kernels take 0 or 1 */
     uint32_t gt_has_alpha;  /* gt is rgba: blend with bg and add the mask loss (utils.py:662-667,681-683) */
+    uint32_t ind_dim;       /* width D of the per-image appearance codes, 0..10 (0 = none).  Read by the *_codes / code entry points; the
+                               plain gather entry points write no code columns, and n2m_s0_render_rounds refuses ind_dim > 0 (it has no
+                               code row: use n2m_s0_render_rounds_codes) */
 } n2m_s0_params;
 
 /* one-time per-process setup (kernel attributes of every stage); call before the first launch / graph capture */
@@ -257,6 +260,63 @@ int n2m_s0_ema_update(const void* table, const void* color_master, const float* 
                       float* shadow_mlp, uint32_t rows, float one_minus_decay, n2m_stream_t stream);
 int n2m_s0_ema_swap(void* table, void* color_master, float* mlp_params, float* shadow_density, void* shadow_color, float* shadow_mlp,
                     uint32_t rows, void* wpack, n2m_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Per-image appearance codes (the reference's --ind_dim D / --ind_num, renderer.py:97-104, network.py:72,159-166).
+ * color_net.0 then reads [xyz | colour features | code of the sample's image]; the code enters the tile image at columns 54..53+D
+ * (1 <= D <= 10, p->ind_dim = D), where W_C1 has room, so every GEMM keeps its shape.  The parameters of the feature live outside the
+ * flat 7648-float MLP vector, in a second block `ind` [64*D + ind_num*D] fp32:
+ *   ind[o*D + j]               = color_net.net.0.weight[o, 35 + j]   (the code columns of the colour net's first layer; lr)
+ *   ind[64*D + i*D + j]        = individual_codes[i, j]              (one code per training image; 0.1 * lr)
+ * with a gradient block g_ind of the same layout (loss-scaled, like g_mlp).  The *_codes entry points are the ones above plus the
+ * code source; with p->ind_dim == 0 they do exactly what the plain ones do.  Code sources:
+ *   codes + ray_img : codes = the [ind_num, D] code table, ray_img [N] int32 = image index of every ray (looked up through the ray id
+ *                     of the march record; indices are not range-checked, as in n2m_s0_gen_rays);
+ *   ray_img == NULL : `codes` points at the ONE code row [D] used for every sample of the launch (evaluation, stage 1).
+ * ---------------------------------------------------------------------------------------- */
+int n2m_s0_encode_fwd_codes(const n2m_s0_params* p, const void* recs, const int32_t* counters, uint32_t Mcap, const float* rays_o,
+                            const float* rays_d, const void* table, const int32_t* offsets, const float* codes, const int32_t* ray_img,
+                            void* enc_tiles, uint32_t part, uint32_t nparts, n2m_stream_t stream);
+/* n2m_s0_encode_points with one code row `code_row` [D] for every point */
+int n2m_s0_encode_points_codes(const n2m_s0_params* p, const float* xyz, const float* dirs, const int32_t* counters, uint32_t Pcap,
+                               const void* table, const int32_t* offsets, const float* code_row, void* enc_tiles, n2m_stream_t stream);
+int n2m_s0_fwd_fused_codes(const n2m_s0_params* p, const void* recs, const int32_t* counters, uint32_t Mcap, const float* rays_o,
+                           const float* rays_d, const void* table, const int32_t* offsets, const float* codes, const int32_t* ray_img,
+                           const void* wpack, void* enc_tiles, void* out, float* spec_sq_sum, n2m_stream_t stream);
+/* n2m_s0_render_rounds with one code row `code_row` [D] for every sample (the reference evaluates with code 0, renderer.py:702-703) */
+int n2m_s0_render_rounds_codes(const n2m_s0_params* p, const float* rays_o, const float* rays_d, const uint8_t* bitfield, uint32_t N,
+                               const uint32_t* schedule, uint32_t num_rounds, float* rays_t, float* rays_far, int32_t* alive, int32_t* ctl,
+                               void* recs, void* enc_tiles, void* out, uint32_t Mcap, const void* table, const int32_t* offsets,
+                               const void* wpack, const float* code_row, float* weights_sum, float* depth, float* image,
+                               n2m_stream_t stream);
+/* n2m_s0_mlp_bwd that also adds the weight gradient of the code columns to g_ind[0 .. 64*D) (loss-scaled, fp32).  The code columns'
+ * input gradient is in denc_tiles columns 54..53+D either way. */
+int n2m_s0_mlp_bwd_codes(const n2m_s0_params* p, const void* enc_tiles, const void* dout, const int32_t* counters, uint32_t Mcap,
+                         const void* wpack, void* denc_tiles, float* g_mlp, float* g_ind, const float* loss_scale, uint32_t part,
+                         uint32_t nparts, n2m_stream_t stream);
+/* code gradient: g_codes[ray_img[n] * D + j] += sum over the samples of ray n of denc[sample, 54 + j] (fp16 loss-scaled terms summed in
+ * fp32; one reduction per ray, one RED per ray and dimension), for the rays of part `part` of `nparts` (rays (offset, count) from the
+ * march), samples below counters[1].  g_codes = g_ind + 64*D.  ray_img NULL: every ray adds into the one row at g_codes.  active_rays
+ * (nullable, = counters + 16 after an adaptive march): the batch is its first n rays.  A non-finite term sets opt_state[3]. */
+int n2m_s0_code_grad(const n2m_s0_params* p, const int32_t* rays, const int32_t* counters, uint32_t N, const void* denc_tiles,
+                     const int32_t* ray_img, float* g_codes, float* opt_state, const int32_t* active_rays, uint32_t part, uint32_t nparts,
+                     n2m_stream_t stream);
+/* the code gradient of a launch with ONE code row (stage 1: the view's image): g_row[j] += sum over the sample rows below counters[1] of
+ * denc[row, 54 + j]; Mcap = the capacity of denc_tiles (sizes the grid).  A non-finite term sets opt_state[3]. */
+int n2m_s0_code_grad_row(const n2m_s0_params* p, const int32_t* counters, uint32_t Mcap, const void* denc_tiles, float* g_row,
+                         float* opt_state, n2m_stream_t stream);
+/* the code columns ind[0 .. 64*D) -> W_C1 columns 54..53+D of wpack (after n2m_s0_pack_weights, which zeroes them) */
+int n2m_s0_pack_code_weights(const float* ind, uint32_t ind_dim, void* wpack, n2m_stream_t stream);
+/* optimizer of the `ind` block (Adam, weight decay 0): `head` ORs a non-finite entry of g_ind[0, n) into found_inf and runs BEFORE
+ * n2m_s0_adam_head; `codes` runs between n2m_s0_adam_head and n2m_s0_adam_post, after n2m_s0_adam_mlp on the same stream (whose repack
+ * zeroes the code columns): it unscales, skips on found_inf, steps the code columns at lr and the codes at 0.1 * lr (renderer.py:173-174),
+ * zeroes g_ind and repacks the code columns into wpack. */
+int n2m_s0_adam_codes_head(const float* g_ind, uint32_t n, float* opt_state, n2m_stream_t stream);
+int n2m_s0_adam_codes(float* ind, float* g_ind, float* m_ind, float* v_ind, uint32_t ind_dim, uint32_t ind_num, void* wpack,
+                      const float* opt_state, float eps, n2m_stream_t stream);
+/* EMA of the `ind` block, as n2m_s0_ema_update / n2m_s0_ema_swap (the swap runs after n2m_s0_ema_swap and repacks the code columns) */
+int n2m_s0_codes_ema_update(const float* ind, float* shadow_ind, uint32_t n, float one_minus_decay, n2m_stream_t stream);
+int n2m_s0_codes_ema_swap(float* ind, float* shadow_ind, uint32_t ind_dim, uint32_t ind_num, void* wpack, n2m_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Data-parallel optimizer fused with its collective over NVLink peer memory (csrc/dp.cu).

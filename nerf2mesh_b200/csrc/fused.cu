@@ -35,10 +35,13 @@ __device__ __forceinline__ void bar_group(uint32_t g) {          // named barrie
     else asm volatile("bar.sync 3, 128;" ::: "memory");
 }
 
+// CODES = false compiles the appearance-code columns out of the gather (include/n2m_b200_fused.h "Per-image appearance codes")
+template <bool CODES>
 __global__ void __launch_bounds__(kFwdThreads, 2)
 k_s0_fwd_fused(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* __restrict__ counters, const float* __restrict__ rays_o,
                const float* __restrict__ rays_d, const TableEntry* __restrict__ table, const int32_t* __restrict__ offsets,
-               const uint8_t* __restrict__ wpack, uint8_t* __restrict__ enc_tiles, float4* __restrict__ out, float* __restrict__ spec_sq_sum) {
+               const uint8_t* __restrict__ wpack, uint8_t* __restrict__ enc_tiles, float4* __restrict__ out, float* __restrict__ spec_sq_sum,
+               const float* __restrict__ codes, const int32_t* __restrict__ ray_img) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ uint64_t bar_full[2], bar_empty[2];
     __shared__ float red[4];
@@ -67,7 +70,8 @@ k_s0_fwd_fused(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* 
         for (uint32_t it = g; it < my_tiles; it += 2, ++k) {
             const uint32_t tile = blockIdx.x + it * gridDim.x;
             float feat[kTileCols];
-            encode_fwd_features<false>(p, recs, rays_o, rays_d, table, offsets, pr, tile * kTile + r, feat);
+            encode_fwd_features<false>(p, recs, rays_o, rays_d, table, offsets, pr, tile * kTile + r, feat, CODES ? codes : nullptr,
+                                       CODES ? ray_img : nullptr);
             // the buffer is free once the TMA store of its previous image has read it and the MLP warps are done with that tile
             if (r == 0) {
                 asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
@@ -115,7 +119,8 @@ k_s0_fwd_fused(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* 
 }  // namespace
 
 cudaError_t fwd_fused_set_attributes() {
-    return cudaFuncSetAttribute(k_s0_fwd_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_BYTES);
+    const cudaError_t e = cudaFuncSetAttribute(k_s0_fwd_fused<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_BYTES);
+    return e != cudaSuccess ? e : cudaFuncSetAttribute(k_s0_fwd_fused<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)FF_BYTES);
 }
 }  // namespace n2m
 
@@ -133,10 +138,27 @@ int n2m_s0_fwd_fused(const n2m_s0_params* p, const void* recs, const int32_t* co
     N2M_REQUIRE(p->num_levels == kLevels, "s0_fwd_fused", "fused path supports num_levels == 16");
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_fwd_fused", "Mcap must be a positive multiple of 128");
     const uint32_t grid = min(Mcap / kTile, (uint32_t)(2 * num_sms()));
-    k_s0_fwd_fused<<<grid, kFwdThreads, FF_BYTES, as_stream(stream)>>>(
+    k_s0_fwd_fused<false><<<grid, kFwdThreads, FF_BYTES, as_stream(stream)>>>(
         *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, static_cast<const TableEntry*>(table), offsets,
-        static_cast<const uint8_t*>(wpack), static_cast<uint8_t*>(enc_tiles), static_cast<float4*>(out), spec_sq_sum);
+        static_cast<const uint8_t*>(wpack), static_cast<uint8_t*>(enc_tiles), static_cast<float4*>(out), spec_sq_sum, nullptr, nullptr);
     return check_launch("s0_fwd_fused");
+}
+
+int n2m_s0_fwd_fused_codes(const n2m_s0_params* p, const void* recs, const int32_t* counters, uint32_t Mcap, const float* rays_o,
+                           const float* rays_d, const void* table, const int32_t* offsets, const float* codes, const int32_t* ray_img,
+                           const void* wpack, void* enc_tiles, void* out, float* spec_sq_sum, n2m_stream_t stream) {
+    N2M_REQUIRE(p && p->ind_dim <= kMaxIndDim, "s0_fwd_fused_codes", "ind_dim must be at most 10");
+    if (p->ind_dim == 0)
+        return n2m_s0_fwd_fused(p, recs, counters, Mcap, rays_o, rays_d, table, offsets, wpack, enc_tiles, out, spec_sq_sum, stream);
+    N2M_REQUIRE(recs && counters && rays_o && rays_d && table && offsets && wpack && enc_tiles && out && codes, "s0_fwd_fused_codes",
+                "null pointer");
+    N2M_REQUIRE(p->num_levels == kLevels, "s0_fwd_fused_codes", "fused path supports num_levels == 16");
+    N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_fwd_fused_codes", "Mcap must be a positive multiple of 128");
+    const uint32_t grid = min(Mcap / kTile, (uint32_t)(2 * num_sms()));
+    k_s0_fwd_fused<true><<<grid, kFwdThreads, FF_BYTES, as_stream(stream)>>>(
+        *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, static_cast<const TableEntry*>(table), offsets,
+        static_cast<const uint8_t*>(wpack), static_cast<uint8_t*>(enc_tiles), static_cast<float4*>(out), spec_sq_sum, codes, ray_img);
+    return check_launch("s0_fwd_fused_codes");
 }
 
 }  // extern "C"

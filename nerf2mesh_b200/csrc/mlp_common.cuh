@@ -25,7 +25,8 @@ constexpr uint32_t W_BYTES = W_P2 + 16 * 32 * 2;    // 25600
 // flat fp32 parameter vector (reference nn.Linear layouts [out, in])
 constexpr uint32_t P_S0 = 0, P_S1 = 608, P_C0 = 640, P_C1 = 2880, P_C2 = 6976, P_P0 = 7360, P_P1 = 7552, P_COUNT = 7648;
 
-// enc tile column -> input index of the first-layer weights (-1: not an input of that net)
+// enc tile column -> input index of the first-layer weights (-1: not an input of that net; the appearance-code columns
+// kColCode.. of color_net.0 live outside the flat vector, see k_pack_code_weights)
 __host__ __device__ __forceinline__ int map_c1(uint32_t k) { return k < 3 ? (int)k : (k >= 19 && k < 51) ? (int)(k - 16) : -1; }
 __host__ __device__ __forceinline__ int map_s1(uint32_t k) { return k < 19 ? (int)k : -1; }
 

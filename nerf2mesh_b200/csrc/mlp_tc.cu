@@ -50,6 +50,15 @@ k_pack_weights(const float* __restrict__ P, uint8_t* __restrict__ wpack) {
     *reinterpret_cast<__half*>(wpack + byte) = __float2half_rn(v);
 }
 
+// appearance-code columns of color_net.0: ind[o * D + j] -> W_C1 (o, 54 + j)
+__global__ void __launch_bounds__(256)
+k_pack_code_weights(const float* __restrict__ ind, uint32_t D, uint8_t* __restrict__ wpack) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= 64 * D) return;
+    const uint32_t o = i / D, j = i % D;
+    *reinterpret_cast<__half*>(wpack + W_C1 + wg::tile_off(o, kColCode + j, 64)) = __float2half_rn(ind[i]);
+}
+
 // ================================================================================================
 // forward
 // ================================================================================================
@@ -419,9 +428,14 @@ __device__ __forceinline__ void for_frag64(const float (&d)[N / 2], uint32_t tid
     for (int i = 0; i < N / 2; ++i) f(frag_row(0, i, tid), frag_col(i, tid), d[i]);
 }
 
-// the weight-gradient accumulators of a CTA -> g_mlp (flat reference layout), atomically
-__device__ __forceinline__ void flush_wgrad(const WgradAcc& wa, float* g_mlp, bool full, uint32_t tid) {
-    for_frag64<64>(wa.c1, tid, [&](uint32_t f, uint32_t o, float v) { const int k = map_c1(f); if (k >= 0) atomicAdd(g_mlp + P_C0 + o * 35 + k, v); });
+// the weight-gradient accumulators of a CTA -> g_mlp (flat reference layout), atomically; with g_ind the appearance-code columns
+// 54..53+D of W_C1 -> g_ind[o * D + (f - 54)] (include/n2m_b200_fused.h "Per-image appearance codes")
+__device__ __forceinline__ void flush_wgrad(const WgradAcc& wa, float* g_mlp, float* g_ind, uint32_t D, bool full, uint32_t tid) {
+    for_frag64<64>(wa.c1, tid, [&](uint32_t f, uint32_t o, float v) {
+        const int k = map_c1(f);
+        if (k >= 0) atomicAdd(g_mlp + P_C0 + o * 35 + k, v);
+        else if (g_ind && f >= kColCode && f < kColCode + D) atomicAdd(g_ind + o * D + (f - kColCode), v);
+    });
     for_frag64<64>(wa.c2, tid, [&](uint32_t f, uint32_t o, float v) { atomicAdd(g_mlp + P_C1 + o * 64 + f, v); });
     for_frag64<16>(wa.c3, tid, [&](uint32_t f, uint32_t o, float v) { if (o < 6) atomicAdd(g_mlp + P_C2 + o * 64 + f, v); });
     for_frag64<32>(wa.s1, tid, [&](uint32_t f, uint32_t o, float v) { const int k = map_s1(f); if (k >= 0) atomicAdd(g_mlp + P_S0 + o * 19 + k, v); });
@@ -471,7 +485,7 @@ __device__ __forceinline__ void mlp_bwd_chain_role(uint32_t c, const n2m_s0_para
 __global__ void __launch_bounds__(kBwdThreads, 1)
 k_mlp_bwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const float4* __restrict__ dout,
           const int32_t* __restrict__ counters, const uint8_t* __restrict__ wpack, uint8_t* __restrict__ denc_tiles,
-          float* __restrict__ g_mlp, const float* __restrict__ loss_scale, uint32_t part, uint32_t nparts) {
+          float* __restrict__ g_mlp, const float* __restrict__ loss_scale, uint32_t part, uint32_t nparts, float* __restrict__ g_ind) {
     extern __shared__ __align__(128) uint8_t smem[];
     __shared__ BwdBars bars;
     const uint32_t tid = threadIdx.x, wgi = tid >> 7;
@@ -517,7 +531,7 @@ k_mlp_bwd(n2m_s0_params p, const uint8_t* __restrict__ enc_tiles, const float4* 
                 if (step == 4) mbar_arrive(&bars.rel[s][REL_SET]);
             }
         }
-        flush_wgrad(wa, g_mlp, full, tid & 127u);
+        flush_wgrad(wa, g_mlp, g_ind, p.ind_dim, full, tid & 127u);
     }
 }
 
@@ -569,8 +583,31 @@ int n2m_s0_mlp_bwd(const n2m_s0_params* p, const void* enc_tiles, const void* do
     const uint32_t grid = min(Mcap / kTile, (uint32_t)num_sms());
     k_mlp_bwd<<<grid, kBwdThreads, B_BYTES, as_stream(stream)>>>(*p, static_cast<const uint8_t*>(enc_tiles), static_cast<const float4*>(dout),
                                                          counters, static_cast<const uint8_t*>(wpack), static_cast<uint8_t*>(denc_tiles),
-                                                         g_mlp, loss_scale, part, nparts);
+                                                         g_mlp, loss_scale, part, nparts, nullptr);
     return check_launch("s0_mlp_bwd");
+}
+
+int n2m_s0_mlp_bwd_codes(const n2m_s0_params* p, const void* enc_tiles, const void* dout, const int32_t* counters, uint32_t Mcap,
+                         const void* wpack, void* denc_tiles, float* g_mlp, float* g_ind, const float* loss_scale, uint32_t part,
+                         uint32_t nparts, n2m_stream_t stream) {
+    N2M_REQUIRE(p && p->ind_dim <= kMaxIndDim, "s0_mlp_bwd_codes", "ind_dim must be at most 10");
+    N2M_REQUIRE(p->ind_dim == 0 || g_ind, "s0_mlp_bwd_codes", "null pointer");
+    N2M_REQUIRE(enc_tiles && dout && counters && wpack && denc_tiles && g_mlp && loss_scale, "s0_mlp_bwd_codes", "null pointer");
+    N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_mlp_bwd_codes", "Mcap must be a positive multiple of 128");
+    N2M_REQUIRE(valid_parts(part, nparts), "s0_mlp_bwd_codes", "nparts must be 1, 2, 4 or 8 and part < nparts");
+    const uint32_t grid = min(Mcap / kTile, (uint32_t)num_sms());
+    k_mlp_bwd<<<grid, kBwdThreads, B_BYTES, as_stream(stream)>>>(*p, static_cast<const uint8_t*>(enc_tiles), static_cast<const float4*>(dout),
+                                                         counters, static_cast<const uint8_t*>(wpack), static_cast<uint8_t*>(denc_tiles),
+                                                         g_mlp, loss_scale, part, nparts, p->ind_dim ? g_ind : nullptr);
+    return check_launch("s0_mlp_bwd_codes");
+}
+
+int n2m_s0_pack_code_weights(const float* ind, uint32_t ind_dim, void* wpack, n2m_stream_t stream) {
+    N2M_REQUIRE(ind_dim <= kMaxIndDim, "s0_pack_code_weights", "ind_dim must be at most 10");
+    if (ind_dim == 0) return 0;
+    N2M_REQUIRE(ind && wpack, "s0_pack_code_weights", "null pointer");
+    k_pack_code_weights<<<div_up(64u * ind_dim, 256u), 256, 0, as_stream(stream)>>>(ind, ind_dim, static_cast<uint8_t*>(wpack));
+    return check_launch("s0_pack_code_weights");
 }
 
 }  // extern "C"

@@ -157,10 +157,81 @@ k_ema_swap(TableEntry* __restrict__ table, float2* __restrict__ cmaster, float* 
     if (i < n_mlp) { const float s = sh_mlp[i]; sh_mlp[i] = mlp[i]; mlp[i] = s; }
 }
 
+// ---- the appearance-code block `ind` [64 D code columns of color_net.0 | ind_num * D codes] (include/n2m_b200_fused.h): two Adam groups,
+// lr and 0.1 lr (renderer.py:173-174), weight decay 0 for both
+__global__ void __launch_bounds__(256)
+k_adam_codes(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v, uint32_t n_cols, uint32_t n,
+             const float* __restrict__ st, float eps) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const bool skip = st[3] != 0.f;
+    const float gi = g[i] * st[7];
+    g[i] = 0.f;
+    if (skip) return;
+    const float lr = i < n_cols ? st[4] : __fmul_rn(st[4], 0.1f);
+    float mi = m[i], vi = v[i];
+    p[i] = adam_update(p[i], gi, mi, vi, __fdiv_rn(lr, st[5]), st[6], eps);
+    m[i] = mi; v[i] = vi;
+}
+
+__global__ void __launch_bounds__(1024)
+k_adam_codes_head(const float* __restrict__ g, uint32_t n, float* __restrict__ st) {
+    int bad = 0;
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) bad |= !isfinite(g[i]);
+    bad = __syncthreads_or(bad);
+    if (threadIdx.x == 0 && bad) st[3] = 1.f;
+}
+
+__global__ void __launch_bounds__(256)
+k_codes_ema(float* __restrict__ p, float* __restrict__ sh, uint32_t n, float one_minus_decay, bool swap) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const float s = sh[i];
+    if (swap) { sh[i] = p[i]; p[i] = s; }
+    else sh[i] = __fsub_rn(s, __fmul_rn(__fsub_rn(s, p[i]), one_minus_decay));
+}
+
 }  // namespace
 }  // namespace n2m
 
 using namespace n2m;
+
+extern "C" int n2m_s0_pack_code_weights(const float* ind, uint32_t ind_dim, void* wpack, n2m_stream_t stream);
+
+extern "C" int n2m_s0_adam_codes_head(const float* g_ind, uint32_t n, float* opt_state, n2m_stream_t stream) {
+    N2M_REQUIRE(g_ind && opt_state, "s0_adam_codes_head", "null pointer");
+    if (n == 0) return 0;
+    k_adam_codes_head<<<1, 1024, 0, as_stream(stream)>>>(g_ind, n, opt_state);
+    return check_launch("s0_adam_codes_head");
+}
+
+extern "C" int n2m_s0_adam_codes(float* ind, float* g_ind, float* m_ind, float* v_ind, uint32_t ind_dim, uint32_t ind_num, void* wpack,
+                                 const float* opt_state, float eps, n2m_stream_t stream) {
+    N2M_REQUIRE(ind_dim <= 10, "s0_adam_codes", "ind_dim must be at most 10");
+    if (ind_dim == 0) return 0;
+    N2M_REQUIRE(ind && g_ind && m_ind && v_ind && wpack && opt_state, "s0_adam_codes", "null pointer");
+    const uint32_t n = (64 + ind_num) * ind_dim;
+    k_adam_codes<<<div_up(n, 256u), 256, 0, as_stream(stream)>>>(ind, g_ind, m_ind, v_ind, 64 * ind_dim, n, opt_state, eps);
+    if (int e = check_launch("s0_adam_codes")) return e;
+    return n2m_s0_pack_code_weights(ind, ind_dim, wpack, stream);
+}
+
+extern "C" int n2m_s0_codes_ema_update(const float* ind, float* shadow_ind, uint32_t n, float one_minus_decay, n2m_stream_t stream) {
+    N2M_REQUIRE(ind && shadow_ind, "s0_codes_ema_update", "null pointer");
+    if (n == 0) return 0;
+    k_codes_ema<<<div_up(n, 256u), 256, 0, as_stream(stream)>>>(const_cast<float*>(ind), shadow_ind, n, one_minus_decay, false);
+    return check_launch("s0_codes_ema_update");
+}
+
+extern "C" int n2m_s0_codes_ema_swap(float* ind, float* shadow_ind, uint32_t ind_dim, uint32_t ind_num, void* wpack, n2m_stream_t stream) {
+    N2M_REQUIRE(ind_dim <= 10, "s0_codes_ema_swap", "ind_dim must be at most 10");
+    if (ind_dim == 0) return 0;
+    N2M_REQUIRE(ind && shadow_ind && wpack, "s0_codes_ema_swap", "null pointer");
+    const uint32_t n = (64 + ind_num) * ind_dim;
+    k_codes_ema<<<div_up(n, 256u), 256, 0, as_stream(stream)>>>(ind, shadow_ind, n, 0.f, true);
+    if (int e = check_launch("s0_codes_ema_swap")) return e;
+    return n2m_s0_pack_code_weights(ind, ind_dim, wpack, stream);
+}
 
 extern "C" int n2m_s0_pack_weights(const float* mlp_params, void* wpack, n2m_stream_t stream);
 extern "C" uint32_t n2m_s0_mlp_param_count(void);

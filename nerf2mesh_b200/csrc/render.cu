@@ -164,6 +164,16 @@ int n2m_s0_render_rounds(const n2m_s0_params* p, const float* rays_o, const floa
                          const uint32_t* schedule, uint32_t num_rounds, float* rays_t, float* rays_far, int32_t* alive, int32_t* ctl,
                          void* recs, void* enc_tiles, void* out, uint32_t Mcap, const void* table, const int32_t* offsets, const void* wpack,
                          float* weights_sum, float* depth, float* image, n2m_stream_t stream) {
+    return n2m_s0_render_rounds_codes(p, rays_o, rays_d, bitfield, N, schedule, num_rounds, rays_t, rays_far, alive, ctl, recs, enc_tiles,
+                                      out, Mcap, table, offsets, wpack, nullptr, weights_sum, depth, image, stream);
+}
+
+int n2m_s0_render_rounds_codes(const n2m_s0_params* p, const float* rays_o, const float* rays_d, const uint8_t* bitfield, uint32_t N,
+                               const uint32_t* schedule, uint32_t num_rounds, float* rays_t, float* rays_far, int32_t* alive, int32_t* ctl,
+                               void* recs, void* enc_tiles, void* out, uint32_t Mcap, const void* table, const int32_t* offsets,
+                               const void* wpack, const float* code_row, float* weights_sum, float* depth, float* image,
+                               n2m_stream_t stream) {
+    N2M_REQUIRE(p && (p->ind_dim == 0 || code_row), "s0_render_rounds", "ind_dim > 0 needs a code row");
     N2M_REQUIRE(p && rays_o && rays_d && bitfield && schedule && rays_t && rays_far && alive && ctl && recs && enc_tiles && out && table &&
                 offsets && wpack && weights_sum && depth && image, "s0_render_rounds", "null pointer");
     N2M_REQUIRE(Mcap % 128 == 0 && Mcap >= N && N > 0, "s0_render_rounds", "Mcap must be a multiple of 128 and >= the chunk's rays");
@@ -174,7 +184,10 @@ int n2m_s0_render_rounds(const n2m_s0_params* p, const float* rays_o, const floa
         if (int e = check_launch("s0_render(plan)")) return e;
         k_r_march<<<div_up(N, 128u), 128, 0, st>>>(*p, rays_o, rays_d, bitfield, rays_t, rays_far, alive, N, ctl, static_cast<float4*>(recs));
         if (int e = check_launch("s0_render(march)")) return e;
-        if (int e = n2m_s0_encode_fwd(p, recs, ctl, Mcap, rays_o, rays_d, table, offsets, enc_tiles, 0, 1, stream)) return e;
+        if (int e = code_row ? n2m_s0_encode_fwd_codes(p, recs, ctl, Mcap, rays_o, rays_d, table, offsets, code_row, nullptr, enc_tiles, 0, 1,
+                                                       stream)
+                             : n2m_s0_encode_fwd(p, recs, ctl, Mcap, rays_o, rays_d, table, offsets, enc_tiles, 0, 1, stream))
+            return e;
         if (int e = n2m_s0_mlp_fwd(p, enc_tiles, ctl, Mcap, wpack, out, nullptr, 0, 1, stream)) return e;
         k_r_composite<<<div_up(N, 128u), 128, 0, st>>>(*p, static_cast<const float4*>(out), static_cast<const float4*>(recs), ctl, alive, N,
                                                       rays_t, weights_sum, depth, image);

@@ -15,7 +15,8 @@ constexpr uint32_t kTile = 128;            // samples per tile image
 constexpr uint32_t kTileCols = 64;         // fp16 features per sample
 constexpr uint32_t kTileBytes = kTile * kTileCols * 2;
 constexpr uint32_t kChunkBytes = kTile * 16;   // one 8-column chunk of a 128-row tile
-constexpr uint32_t kColXyz = 0, kColDens = 3, kColColor = 19, kColDir = 51;
+constexpr uint32_t kColXyz = 0, kColDens = 3, kColColor = 19, kColDir = 51, kColCode = 54;
+constexpr uint32_t kMaxIndDim = kTileCols - kColCode;      // appearance-code columns the tile image has room for
 constexpr uint32_t kLevels = 16;
 
 struct __align__(8) TableEntry { float d; __half2 c; };
@@ -138,14 +139,18 @@ __device__ __forceinline__ uint32_t pack2(float a, float b) {
 }
 
 // ---- gather of one sample: the 64 fp16 columns of its tile-image row (xyz | 16 density features | 32 colour features | unit direction
-// | zeros), shared by the stand-alone gather kernel (stage0.cu) and the fused forward kernel (fused.cu).  POINTS = false: the sample
-// comes from march record j; POINTS = true: explicit position rays_o[j] / direction rays_d[j] (density-grid update, stage 1, tests).
+// | p.ind_dim appearance-code columns | zeros), shared by the stand-alone gather kernel (stage0.cu) and the fused forward kernel (fused.cu).
+// POINTS = false: the sample comes from march record j; POINTS = true: explicit position rays_o[j] / direction rays_d[j] (density-grid
+// update, stage 1, tests).  Codes (include/n2m_b200_fused.h "Per-image appearance codes"): none when `codes` is null, else row
+// ray_img[ray of record j] of the code table `codes`, or the one row at `codes` when ray_img is null; rounded to fp16 by the tile store
+// as autocast rounds the concatenated input of color_net.0.
 // Returns false when row j is outside [pr.lo, pr.hi) (a row of another part, or past the last sample: all zeros). ----
 template <bool POINTS>
 __device__ __forceinline__ bool
 encode_fwd_features(const n2m_s0_params& p, const float4* __restrict__ recs, const float* __restrict__ rays_o,
                     const float* __restrict__ rays_d, const TableEntry* __restrict__ table, const int32_t* __restrict__ offsets,
-                    const PartRange pr, uint32_t j, float (&feat)[kTileCols]) {
+                    const PartRange pr, uint32_t j, float (&feat)[kTileCols], const float* __restrict__ codes = nullptr,
+                    const int32_t* __restrict__ ray_img = nullptr) {
 #pragma unroll
     for (uint32_t i = 0; i < kTileCols; ++i) feat[i] = 0.f;
     Sample s;
@@ -191,6 +196,15 @@ encode_fwd_features(const n2m_s0_params& p, const float4* __restrict__ recs, con
             feat[kColColor + 2 * l] = c0;
             feat[kColColor + 2 * l + 1] = c1;
         }
+    }
+    // after the level walk, so that the code columns hold no register across it
+    if (codes && own) {
+        const uint32_t D = p.ind_dim;
+        const float* row = codes;
+        if (!POINTS && ray_img) row += (size_t)ray_img[__float_as_int(recs[j].w)] * D;
+#pragma unroll
+        for (uint32_t k = 0; k < kMaxIndDim; ++k)
+            if (k < D) feat[kColCode + k] = __ldg(row + k);
     }
     return own;
 }

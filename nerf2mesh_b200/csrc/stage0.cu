@@ -269,27 +269,124 @@ __device__ __forceinline__ void
 encode_fwd_tile(const n2m_s0_params& p, const float4* __restrict__ recs,
                 const float* __restrict__ rays_o, const float* __restrict__ rays_d,
                 const TableEntry* __restrict__ table, const int32_t* __restrict__ offsets,
-                uint8_t* __restrict__ enc_tiles, const PartRange pr, uint32_t nparts, uint32_t tile) {
+                uint8_t* __restrict__ enc_tiles, const PartRange pr, uint32_t nparts, uint32_t tile,
+                const float* __restrict__ codes, const int32_t* __restrict__ ray_img) {
     float feat[kTileCols];
-    const bool own = encode_fwd_features<POINTS>(p, recs, rays_o, rays_d, table, offsets, pr, tile * kTile + threadIdx.x, feat);
+    const bool own = encode_fwd_features<POINTS>(p, recs, rays_o, rays_d, table, offsets, pr, tile * kTile + threadIdx.x, feat, codes,
+                                                 ray_img);
     if (nparts > 1 && !own) return;                  // (whole-batch mode also zero-fills the rows past M of the last tile)
     store_tile_row(enc_tiles + (size_t)tile * kTileBytes, threadIdx.x, feat);
 }
 
 // one block per 128-sample tile of the part's range [lo, hi) (grid-stride, so any grid size is correct: the host sizes
-// the grid for the expected share of the part and the loop covers an unbalanced one)
-template <bool POINTS>
+// the grid for the expected share of the part and the loop covers an unbalanced one).  CODES = false compiles the code columns out
+// (the kernel without appearance codes is the one it was before they existed).
+template <bool POINTS, bool CODES>
 __global__ void __launch_bounds__(kTile, 6)
 k_s0_encode_fwd(n2m_s0_params p, const float4* __restrict__ recs, const int32_t* __restrict__ counters,
                 const float* __restrict__ rays_o, const float* __restrict__ rays_d,
                 const TableEntry* __restrict__ table, const int32_t* __restrict__ offsets,
-                uint8_t* __restrict__ enc_tiles, uint32_t part, uint32_t nparts) {
+                uint8_t* __restrict__ enc_tiles, uint32_t part, uint32_t nparts, const float* __restrict__ codes,
+                const int32_t* __restrict__ ray_img) {
     const PartRange pr = part_range(counters, part, nparts);
     if (pr.hi <= pr.lo) return;
     const uint32_t t1 = (pr.hi + kTile - 1) / kTile;
 #pragma unroll 1
     for (uint32_t tile = pr.lo / kTile + blockIdx.x; tile < t1; tile += gridDim.x)
-        encode_fwd_tile<POINTS>(p, recs, rays_o, rays_d, table, offsets, enc_tiles, pr, nparts, tile);
+        encode_fwd_tile<POINTS>(p, recs, rays_o, rays_d, table, offsets, enc_tiles, pr, nparts, tile, CODES ? codes : nullptr,
+                                CODES ? ray_img : nullptr);
+}
+
+// ------------------------------------------------------------------------------------------------
+// appearance-code gradient (n2m_s0_code_grad): one warp per ray.  The ray's samples are contiguous rows of denc_tiles; every lane sums
+// the code columns of every 32nd sample in fp32, the warp reduces, lane j < D issues the ray's one RED for dimension j.  Samples of a
+// ray share its image, so the REDs are per ray and not per sample: with random_image_batch 4096 rays fall on ~100 code rows.
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(128)
+k_s0_code_grad(uint32_t D, const int32_t* __restrict__ rays, const int32_t* __restrict__ counters, uint32_t N,
+               const uint8_t* __restrict__ denc_tiles, const int32_t* __restrict__ ray_img, float* __restrict__ g_codes,
+               float* __restrict__ opt_state, const int32_t* __restrict__ active_rays, uint32_t e0, uint32_t e1) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t n_act = ray_count(active_rays, N);
+    const uint32_t ray_lo = part_first_ray(n_act, e0), ray_hi = part_first_ray(n_act, e1);
+    const uint32_t M = (uint32_t)counters[1];                 // rows past the sample capacity hold no sample
+    bool bad = false;
+    for (uint32_t n = ray_lo + ((blockIdx.x * blockDim.x + threadIdx.x) >> 5); n < ray_hi; n += (gridDim.x * blockDim.x) >> 5) {
+        const uint32_t off = (uint32_t)rays[2 * n], end = min(off + (uint32_t)rays[2 * n + 1], M);
+        float acc[kMaxIndDim];
+#pragma unroll
+        for (uint32_t k = 0; k < kMaxIndDim; ++k) acc[k] = 0.f;
+        for (uint32_t j = off + lane; j < end; j += 32) {
+            const uint8_t* row = denc_tiles + (size_t)(j / kTile) * kTileBytes + (j % kTile) * 16;
+            // columns 54, 55 are the last word of chunk 6, columns 56..63 all of chunk 7
+            const uint32_t w6 = __ldg(reinterpret_cast<const uint32_t*>(row + 6 * kChunkBytes + 12));
+            const uint4 w7 = D > 2 ? __ldg(reinterpret_cast<const uint4*>(row + 7 * kChunkBytes)) : make_uint4(0, 0, 0, 0);
+            const uint32_t w[5] = {w6, w7.x, w7.y, w7.z, w7.w};
+#pragma unroll
+            for (uint32_t k = 0; k < kMaxIndDim; ++k) {
+                if (k < D) {
+                    const __half2 h = *reinterpret_cast<const __half2*>(&w[k / 2]);
+                    const float v = (k & 1) ? __high2float(h) : __low2float(h);
+                    bad |= !isfinite(v);
+                    acc[k] += v;
+                }
+            }
+        }
+        float* dst = ray_img ? g_codes + (size_t)ray_img[n] * D : g_codes;
+#pragma unroll
+        for (uint32_t k = 0; k < kMaxIndDim; ++k) {
+            if (k < D) {
+                float v = acc[k];
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+                if (lane == k && end > off) atomicAdd(dst + k, v);
+            }
+        }
+    }
+    if (__any_sync(0xffffffffu, bad) && lane == 0) opt_state[3] = 1.f;
+}
+
+// the same sum when ONE code row serves the whole launch (stage 1: one view, one image): every sample row below counters[1] adds into
+// g_row; each thread sums a grid-stride share of the rows, the CTA reduces, one RED per CTA and dimension
+__global__ void __launch_bounds__(256)
+k_s0_code_grad_row(uint32_t D, const int32_t* __restrict__ counters, const uint8_t* __restrict__ denc_tiles, float* __restrict__ g_row,
+                   float* __restrict__ opt_state) {
+    __shared__ float red[8][kMaxIndDim];
+    const uint32_t M = (uint32_t)counters[1];
+    const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float acc[kMaxIndDim];
+#pragma unroll
+    for (uint32_t k = 0; k < kMaxIndDim; ++k) acc[k] = 0.f;
+    bool bad = false;
+    for (uint32_t j = blockIdx.x * blockDim.x + threadIdx.x; j < M; j += gridDim.x * blockDim.x) {
+        const uint8_t* row = denc_tiles + (size_t)(j / kTile) * kTileBytes + (j % kTile) * 16;
+        const uint32_t w6 = __ldg(reinterpret_cast<const uint32_t*>(row + 6 * kChunkBytes + 12));
+        const uint4 w7 = D > 2 ? __ldg(reinterpret_cast<const uint4*>(row + 7 * kChunkBytes)) : make_uint4(0, 0, 0, 0);
+        const uint32_t w[5] = {w6, w7.x, w7.y, w7.z, w7.w};
+#pragma unroll
+        for (uint32_t k = 0; k < kMaxIndDim; ++k) {
+            if (k < D) {
+                const __half2 h = *reinterpret_cast<const __half2*>(&w[k / 2]);
+                const float v = (k & 1) ? __high2float(h) : __low2float(h);
+                bad |= !isfinite(v);
+                acc[k] += v;
+            }
+        }
+    }
+#pragma unroll
+    for (uint32_t k = 0; k < kMaxIndDim; ++k) {
+        float v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) red[warp][k] = v;
+    }
+    bad = __syncthreads_or(bad);
+    if (threadIdx.x < D) {
+        float v = 0.f;
+        for (uint32_t w_ = 0; w_ < blockDim.x / 32; ++w_) v += red[w_][threadIdx.x];
+        atomicAdd(g_row + threadIdx.x, v);
+    }
+    if (threadIdx.x == 0 && bad) opt_state[3] = 1.f;
 }
 
 // TV gradient of the density feature at one lattice cell of one level (gridencoder.cu:506-609), times weight w: centre, +1
@@ -933,10 +1030,52 @@ int n2m_s0_encode_fwd(const n2m_s0_params* p, const void* recs, const int32_t* c
     N2M_REQUIRE(p->num_levels == kLevels, "s0_encode_fwd", "fused path supports num_levels == 16");
     N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_encode_fwd", "Mcap must be a positive multiple of 128");
     N2M_REQUIRE(valid_parts(part, nparts), "s0_encode_fwd", "nparts must be 1, 2, 4 or 8 and part < nparts");
-    k_s0_encode_fwd<false><<<part_grid(Mcap, nparts), kTile, 0, as_stream(stream)>>>(*p, static_cast<const float4*>(recs), counters, rays_o, rays_d,
-                                                                                   static_cast<const TableEntry*>(table), offsets,
-                                                                                   static_cast<uint8_t*>(enc_tiles), part, nparts);
+    k_s0_encode_fwd<false, false><<<part_grid(Mcap, nparts), kTile, 0, as_stream(stream)>>>(
+        *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, static_cast<const TableEntry*>(table), offsets,
+        static_cast<uint8_t*>(enc_tiles), part, nparts, nullptr, nullptr);
     return check_launch("s0_encode_fwd");
+}
+
+int n2m_s0_encode_fwd_codes(const n2m_s0_params* p, const void* recs, const int32_t* counters, uint32_t Mcap, const float* rays_o,
+                            const float* rays_d, const void* table, const int32_t* offsets, const float* codes, const int32_t* ray_img,
+                            void* enc_tiles, uint32_t part, uint32_t nparts, n2m_stream_t stream) {
+    N2M_REQUIRE(p && p->ind_dim <= kMaxIndDim, "s0_encode_fwd_codes", "ind_dim must be at most 10");
+    if (p->ind_dim == 0) return n2m_s0_encode_fwd(p, recs, counters, Mcap, rays_o, rays_d, table, offsets, enc_tiles, part, nparts, stream);
+    N2M_REQUIRE(recs && counters && rays_o && rays_d && table && offsets && enc_tiles && codes, "s0_encode_fwd_codes", "null pointer");
+    N2M_REQUIRE(p->num_levels == kLevels, "s0_encode_fwd_codes", "fused path supports num_levels == 16");
+    N2M_REQUIRE(Mcap % kTile == 0 && Mcap > 0, "s0_encode_fwd_codes", "Mcap must be a positive multiple of 128");
+    N2M_REQUIRE(valid_parts(part, nparts), "s0_encode_fwd_codes", "nparts must be 1, 2, 4 or 8 and part < nparts");
+    k_s0_encode_fwd<false, true><<<part_grid(Mcap, nparts), kTile, 0, as_stream(stream)>>>(
+        *p, static_cast<const float4*>(recs), counters, rays_o, rays_d, static_cast<const TableEntry*>(table), offsets,
+        static_cast<uint8_t*>(enc_tiles), part, nparts, codes, ray_img);
+    return check_launch("s0_encode_fwd_codes");
+}
+
+int n2m_s0_code_grad_row(const n2m_s0_params* p, const int32_t* counters, uint32_t Mcap, const void* denc_tiles, float* g_row,
+                         float* opt_state, n2m_stream_t stream) {
+    N2M_REQUIRE(p && p->ind_dim <= kMaxIndDim, "s0_code_grad_row", "ind_dim must be at most 10");
+    if (p->ind_dim == 0 || Mcap == 0) return 0;
+    N2M_REQUIRE(counters && denc_tiles && g_row && opt_state, "s0_code_grad_row", "null pointer");
+    const uint32_t grid = min(div_up(Mcap, 256u * 8u), (uint32_t)(4 * num_sms()));
+    k_s0_code_grad_row<<<grid, 256, 0, as_stream(stream)>>>(p->ind_dim, counters, static_cast<const uint8_t*>(denc_tiles), g_row, opt_state);
+    return check_launch("s0_code_grad_row");
+}
+
+int n2m_s0_code_grad(const n2m_s0_params* p, const int32_t* rays, const int32_t* counters, uint32_t N, const void* denc_tiles,
+                     const int32_t* ray_img, float* g_codes, float* opt_state, const int32_t* active_rays, uint32_t part, uint32_t nparts,
+                     n2m_stream_t stream) {
+    N2M_REQUIRE(p && p->ind_dim <= kMaxIndDim, "s0_code_grad", "ind_dim must be at most 10");
+    N2M_REQUIRE(valid_parts(part, nparts), "s0_code_grad", "nparts must be 1, 2, 4 or 8 and part < nparts");
+    if (p->ind_dim == 0 || N == 0) return 0;
+    N2M_REQUIRE(rays && counters && denc_tiles && g_codes && opt_state, "s0_code_grad", "null pointer");
+    const uint32_t e0 = part * kPartSlots / nparts, e1 = (part + 1) * kPartSlots / nparts;
+    // the part's rays may be known on the device only (adaptive count): cover the largest part any n <= N gives
+    const uint32_t most = active_rays ? div_up(N, nparts) + 1 : part_first_ray(N, e1) - part_first_ray(N, e0);
+    if (most == 0) return 0;
+    k_s0_code_grad<<<div_up(most * 32u, 128u), 128, 0, as_stream(stream)>>>(p->ind_dim, rays, counters, N,
+                                                                          static_cast<const uint8_t*>(denc_tiles), ray_img, g_codes,
+                                                                          opt_state, active_rays, e0, e1);
+    return check_launch("s0_code_grad");
 }
 
 int n2m_s0_encode_points(const n2m_s0_params* p, const float* xyz, const float* dirs, const int32_t* counters, uint32_t Pcap,
@@ -944,10 +1083,23 @@ int n2m_s0_encode_points(const n2m_s0_params* p, const float* xyz, const float* 
     N2M_REQUIRE(p && xyz && counters && table && offsets && enc_tiles, "s0_encode_points", "null pointer");
     N2M_REQUIRE(p->num_levels == kLevels, "s0_encode_points", "fused path supports num_levels == 16");
     N2M_REQUIRE(Pcap % kTile == 0 && Pcap > 0, "s0_encode_points", "Pcap must be a positive multiple of 128");
-    k_s0_encode_fwd<true><<<Pcap / kTile, kTile, 0, as_stream(stream)>>>(*p, nullptr, counters, xyz, dirs,
-                                                                         static_cast<const TableEntry*>(table), offsets,
-                                                                         static_cast<uint8_t*>(enc_tiles), 0, 1);
+    k_s0_encode_fwd<true, false><<<Pcap / kTile, kTile, 0, as_stream(stream)>>>(*p, nullptr, counters, xyz, dirs,
+                                                                                static_cast<const TableEntry*>(table), offsets,
+                                                                                static_cast<uint8_t*>(enc_tiles), 0, 1, nullptr, nullptr);
     return check_launch("s0_encode_points");
+}
+
+int n2m_s0_encode_points_codes(const n2m_s0_params* p, const float* xyz, const float* dirs, const int32_t* counters, uint32_t Pcap,
+                               const void* table, const int32_t* offsets, const float* code_row, void* enc_tiles, n2m_stream_t stream) {
+    N2M_REQUIRE(p && p->ind_dim <= kMaxIndDim, "s0_encode_points_codes", "ind_dim must be at most 10");
+    if (p->ind_dim == 0) return n2m_s0_encode_points(p, xyz, dirs, counters, Pcap, table, offsets, enc_tiles, stream);
+    N2M_REQUIRE(xyz && counters && table && offsets && enc_tiles && code_row, "s0_encode_points_codes", "null pointer");
+    N2M_REQUIRE(p->num_levels == kLevels, "s0_encode_points_codes", "fused path supports num_levels == 16");
+    N2M_REQUIRE(Pcap % kTile == 0 && Pcap > 0, "s0_encode_points_codes", "Pcap must be a positive multiple of 128");
+    k_s0_encode_fwd<true, true><<<Pcap / kTile, kTile, 0, as_stream(stream)>>>(*p, nullptr, counters, xyz, dirs,
+                                                                               static_cast<const TableEntry*>(table), offsets,
+                                                                               static_cast<uint8_t*>(enc_tiles), 0, 1, code_row, nullptr);
+    return check_launch("s0_encode_points_codes");
 }
 
 int n2m_s0_grid_points(uint32_t H, uint32_t first_cell, uint32_t count, float cas_bound, const float* noise, float* xyz,

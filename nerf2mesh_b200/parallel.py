@@ -12,6 +12,8 @@ class GradSync:
     opt_state) over the default process group; found_inf is OR-ed so every rank skips the same steps."""
 
     def __init__(self, trainer, group=None):
+        if getattr(trainer, "ind_dim", 0):
+            raise ValueError("data-parallel training with appearance codes (ind_dim > 0) is not supported")
         self.t = trainer
         self.group = group
         self.world = dist.get_world_size(group)
@@ -71,6 +73,8 @@ class PeerAdam:
     fused = True
 
     def __init__(self, trainer, group=None):
+        if getattr(trainer, "ind_dim", 0):
+            raise ValueError("data-parallel training with appearance codes (ind_dim > 0) is not supported")
         t = self.t = trainer
         self.group = group
         self.world = W = dist.get_world_size(group)
@@ -168,6 +172,8 @@ class NvlsAdam(PeerAdam):
     kernel.  Raises when the fabric / driver offers no multicast (callers fall back to PeerAdam, then to NCCL)."""
 
     def __init__(self, trainer, group=None):
+        if getattr(trainer, "ind_dim", 0):
+            raise ValueError("data-parallel training with appearance codes (ind_dim > 0) is not supported")
         import torch.distributed._symmetric_memory as symm_mem
         t = self.t = trainer
         self.group = group

@@ -28,7 +28,7 @@ class S0Params(ctypes.Structure):
     _fields_ = [(n, c_float) for n in ("bound", "grid_bound", "inv_2gb", "dt_gamma", "min_near", "T_thresh", "S",
                                        "lambda_mask", "lambda_specular", "lambda_tv", "lambda_entropy")] + \
                [(n, c_uint32) for n in ("contract", "max_steps", "cascades", "grid_size", "num_levels", "base_res",
-                                        "shading_full", "gt_has_alpha")]
+                                        "shading_full", "gt_has_alpha", "ind_dim")]
 
 
 PP = ctypes.POINTER(S0Params)
@@ -65,6 +65,18 @@ _lib.register({
     "n2m_s0_render_finish": [P, P, P, F, U, P],
     "n2m_s0_ema_update": [P, P, P, P, P, P, U, F, P],
     "n2m_s0_ema_swap": [P, P, P, P, P, P, U, P, P],
+    "n2m_s0_encode_fwd_codes": [PP, P, P, U, P, P, P, P, P, P, P, U, U, P],
+    "n2m_s0_encode_points_codes": [PP, P, P, P, U, P, P, P, P, P],
+    "n2m_s0_fwd_fused_codes": [PP, P, P, U, P, P, P, P, P, P, P, P, P, P, P],
+    "n2m_s0_render_rounds_codes": [PP, P, P, P, U, P, U, P, P, P, P, P, P, P, U, P, P, P, P, P, P, P, P],
+    "n2m_s0_mlp_bwd_codes": [PP, P, P, P, U, P, P, P, P, P, U, U, P],
+    "n2m_s0_code_grad": [PP, P, P, U, P, P, P, P, P, U, U, P],
+    "n2m_s0_code_grad_row": [PP, P, U, P, P, P, P],
+    "n2m_s0_pack_code_weights": [P, U, P, P],
+    "n2m_s0_adam_codes_head": [P, U, P, P],
+    "n2m_s0_adam_codes": [P, P, P, P, U, U, P, P, F, P],
+    "n2m_s0_codes_ema_update": [P, P, U, F, P],
+    "n2m_s0_codes_ema_swap": [P, P, U, U, P, P],
 })
 _lib.lib.n2m_s0_wpack_bytes.restype = c_uint32
 _lib.lib.n2m_s0_mlp_param_count.restype = c_uint32
@@ -75,6 +87,8 @@ MLP_LAYOUT = [
     ("color_net.net.0.weight", (64, 35)), ("color_net.net.1.weight", (64, 64)), ("color_net.net.2.weight", (6, 64)),
     ("specular_net.net.0.weight", (32, 6)), ("specular_net.net.1.weight", (3, 32)),
 ]
+# per-image appearance codes (include/n2m_b200_fused.h "Per-image appearance codes"): widest code the 64-column tile image has room for
+MAX_IND_DIM = 10
 
 
 class Stage0Config:
@@ -83,7 +97,7 @@ class Stage0Config:
     def __init__(self, bound=1.0, contract=False, dt_gamma=0.0, max_steps=1024, grid_size=128, min_near=0.05,
                  T_thresh=1e-4, num_levels=16, base_resolution=16, log2_hashmap_size=19, lambda_mask=0.1,
                  lambda_specular=1e-5, lambda_tv=1e-8, lambda_entropy=0.0, lr=1e-2, eps=1e-15, max_samples=None, num_rays=4096,
-                 loss_scale=65536.0, adaptive_num_rays=False, num_points=2 ** 18, max_rays=None):
+                 loss_scale=65536.0, adaptive_num_rays=False, num_points=2 ** 18, max_rays=None, ind_dim=0, ind_num=500):
         self.real_bound = float(bound)
         self.contract = bool(contract)
         self.bound = 2.0 if contract else float(bound)          # renderer.py:74-80
@@ -114,6 +128,14 @@ class Stage0Config:
         self.max_samples = int(max_samples) if max_samples else self.num_rays * 128
         self.max_samples = (self.max_samples + 127) // 128 * 128
         self.loss_scale = float(loss_scale)
+        # --ind_dim / --ind_num (main.py:94-95): a learned code per training image, appended to color_net's input
+        # (renderer.py:97-104, network.py:72,159-166).  The code columns share the colour net's 64-column first GEMM with the features,
+        # so at most MAX_IND_DIM of them fit.
+        self.ind_dim, self.ind_num = int(ind_dim), int(ind_num)
+        if not 0 <= self.ind_dim <= MAX_IND_DIM:
+            raise ValueError(f"ind_dim must be in [0, {MAX_IND_DIM}], got {self.ind_dim}")
+        if self.ind_num < 1:
+            raise ValueError(f"ind_num must be at least 1, got {self.ind_num}")
 
 
 class _Slot:
@@ -128,7 +150,15 @@ class _Slot:
         self.tbuf = torch.empty(N * max_steps * 2, device=dev)
         self.recs = torch.zeros(Mc, 4, device=dev)
         self.cam_nf = torch.zeros(N, 2, device=dev)                      # per-ray (near, far) clamp, renderer.py:689-691
+        self.ray_img = torch.zeros(N, dtype=torch.int32, device=dev)     # image index of every ray (appearance codes only)
         self.has_alpha = True
+
+    def load_index(self, index):
+        """The batch's image indices (data['index']): an int for the whole batch, or an int32 [N] tensor, one per ray."""
+        if isinstance(index, int):
+            self.ray_img.fill_(index)
+        else:
+            self.ray_img.copy_(index, non_blocking=True)
 
     def load(self, rays_o, rays_d, gt, bg, noises=None, cam_near_far=None):
         N = self.rays_o.shape[0]
@@ -150,6 +180,10 @@ class Stage0Trainer:
     # adaptive ray count (Stage0Config.adaptive_num_rays): the device-resident control block the march reads and rewrites
     adaptive = False
     ray_ctl = None
+    # per-image appearance codes (Stage0Config.ind_dim > 0): the parameter block `ind` [64 D code columns of color_net.0 | ind_num D codes]
+    # (include/n2m_b200_fused.h "Per-image appearance codes") with its gradient g_ind and Adam moments m_ind / v_ind
+    ind_dim = 0
+    ind_num = 0
     _ray_ctl_undo = None        # ray_ctl as it was before the side-stream march of a prefetched batch (see drop_prefetch)
 
     def __init__(self, cfg: Stage0Config, device="cuda", seed=0):
@@ -175,6 +209,11 @@ class Stage0Trainer:
         self.g_mlps = [torch.zeros_like(self.mlp)]
         self.m_mlp = torch.zeros_like(self.mlp); self.v_mlp = torch.zeros_like(self.mlp)
         self.wpack = torch.zeros(int(_lib.lib.n2m_s0_wpack_bytes()), dtype=torch.uint8, device=dev)
+        if c.ind_dim:
+            self.ind_dim, self.ind_num = c.ind_dim, c.ind_num
+            self.ind = torch.zeros((64 + c.ind_num) * c.ind_dim, dtype=torch.float32, device=dev)
+            self.g_ind = torch.zeros_like(self.ind)
+            self.m_ind = torch.zeros_like(self.ind); self.v_ind = torch.zeros_like(self.ind)
         self.opt_state = torch.zeros(8, dtype=torch.float32, device=dev)
         self.opt_state[0] = c.loss_scale
         self.opt_state[4] = c.lr
@@ -287,6 +326,7 @@ class Stage0Trainer:
         p.contract, p.max_steps, p.cascades, p.grid_size = int(c.contract), c.max_steps, c.cascade, c.grid_size
         p.num_levels, p.base_res = c.num_levels, c.base_resolution
         p.shading_full, p.gt_has_alpha = int(shading_full), int(gt_has_alpha)
+        p.ind_dim = self.ind_dim
 
     def params_with(self, **fields):
         """A copy of `params` with `fields` overridden, e.g. params_with(shading_full=0) for sigma-only evaluation."""
@@ -303,8 +343,12 @@ class Stage0Trainer:
         state = {"encoder.embeddings": torch.rand(self.rows, 1, generator=g) * 2e-4 - 1e-4,
                  "encoder_color.embeddings": torch.rand(self.rows, 2, generator=g) * 2e-4 - 1e-4}
         for name, (o, i) in MLP_LAYOUT:
+            if name == "color_net.net.0.weight":
+                i += self.ind_dim                   # the code columns are inputs of the same nn.Linear (network.py:72)
             k = 1.0 / math.sqrt(i)
             state[name] = (torch.rand(o, i, generator=g) * 2 - 1) * k
+        if self.ind_dim:
+            state["individual_codes"] = torch.randn(self.ind_num, self.ind_dim, generator=g) * 0.1     # renderer.py:101-102
         self.load_reference_state(state)
 
     def load_reference_state(self, state):
@@ -313,10 +357,21 @@ class Stage0Trainer:
         ec = state["encoder_color.embeddings"].to(dev, torch.float32).contiguous()
         assert ed.shape == (self.rows, 1) and ec.shape == (self.rows, 2)
         call("n2m_s0_pack_tables", ptr(ed), ptr(ec), self.rows, ptr(self.table), ptr(self.color_master), stream())
-        flat = torch.cat([state[n].to(dev, torch.float32).reshape(-1) for n, _ in MLP_LAYOUT])
+        D = self.ind_dim
+        c0 = state["color_net.net.0.weight"]
+        if tuple(c0.shape) != (64, 35 + D):
+            raise ValueError(f"color_net.net.0.weight has shape {tuple(c0.shape)}, the model (ind_dim = {D}) expects {(64, 35 + D)}")
+        flat = torch.cat([(state[n][:, :35] if n == "color_net.net.0.weight" else state[n]).to(dev, torch.float32).reshape(-1)
+                          for n, _ in MLP_LAYOUT])
         assert flat.numel() == self.n_mlp
         self.mlp.copy_(flat)
         call("n2m_s0_pack_weights", ptr(self.mlp), ptr(self.wpack), stream())
+        if D:
+            codes = state["individual_codes"]
+            if tuple(codes.shape) != (self.ind_num, D):
+                raise ValueError(f"individual_codes has shape {tuple(codes.shape)}, the model expects {(self.ind_num, D)}")
+            self.ind.copy_(torch.cat([c0[:, 35:].to(dev, torch.float32).reshape(-1), codes.to(dev, torch.float32).reshape(-1)]))
+            call("n2m_s0_pack_code_weights", ptr(self.ind), D, ptr(self.wpack), stream())
         if "density_bitfield" in state:
             self.density_bitfield.copy_(state["density_bitfield"].to(dev))
         if "density_grid" in state:
@@ -338,7 +393,22 @@ class Stage0Trainer:
         for name, shp in MLP_LAYOUT:
             n = shp[0] * shp[1]
             state[name] = self.mlp[o:o + n].view(shp).clone(); o += n
+        if self.ind_dim:
+            self._with_codes(state, self.ind)
         return state
+
+    def _with_codes(self, tensors, ind):
+        """Reference layout of an `ind` block (parameters, gradients or EMA shadow) merged into `tensors`: the code columns appended to
+        color_net.net.0.weight ([64, 35 + D]) and individual_codes [ind_num, D] (renderer.py:102)."""
+        D = self.ind_dim
+        key = "color_net.net.0.weight"
+        tensors[key] = torch.cat([tensors[key], ind[:64 * D].view(64, D)], dim=1)
+        tensors["individual_codes"] = ind[64 * D:].view(self.ind_num, D).clone()
+        return tensors
+
+    def _codes_table(self):
+        """Device address of the code table [ind_num, D] (row 0: the code the reference evaluates with, renderer.py:702-703)."""
+        return self.ind.data_ptr() + 4 * 64 * self.ind_dim
 
     def save_reference_checkpoint(self, path, epoch=0, stats=None, best=False, full=False):
         """A checkpoint in the schema `Trainer.save_checkpoint` writes and `Trainer.load_checkpoint` reads (nerf/utils.py:1345-1381,
@@ -369,6 +439,8 @@ class Stage0Trainer:
         st = self.export_reference_state()
         self._ema = {"d": st["encoder.embeddings"].reshape(-1).contiguous(), "c": st["encoder_color.embeddings"].contiguous(),
                      "mlp": self.mlp.clone()}
+        if self.ind_dim:
+            self._ema["ind"] = self.ind.clone()
 
     def ema_update(self):
         """`self.ema.update()` -- the reference calls it once per EPOCH (utils.py:1213-1214), not per step.  torch_ema's warm-up:
@@ -379,11 +451,15 @@ class Stage0Trainer:
         e = self._ema
         call("n2m_s0_ema_update", ptr(self.table), ptr(self.color_master), ptr(self.mlp), ptr(e["d"]), ptr(e["c"]), ptr(e["mlp"]),
              self.rows, 1.0 - decay, stream())
+        if self.ind_dim:
+            call("n2m_s0_codes_ema_update", ptr(self.ind), ptr(e["ind"]), self.ind.numel(), 1.0 - decay, stream())
 
     def _ema_swap(self):
         e = self._ema
         call("n2m_s0_ema_swap", ptr(self.table), ptr(self.color_master), ptr(self.mlp), ptr(e["d"]), ptr(e["c"]), ptr(e["mlp"]),
              self.rows, ptr(self.wpack), stream())
+        if self.ind_dim:        # after the swap above, whose repack zeroes the code columns
+            call("n2m_s0_codes_ema_swap", ptr(self.ind), ptr(e["ind"]), self.ind_dim, self.ind_num, ptr(self.wpack), stream())
         self._ema_swapped = not self._ema_swapped
 
     def ema_apply(self):
@@ -410,6 +486,10 @@ class Stage0Trainer:
                  "color_net.net.0.weight", "color_net.net.1.weight", "color_net.net.2.weight",
                  "specular_net.net.0.weight", "specular_net.net.1.weight"]
         tensors = {"encoder.embeddings": e["d"].view(-1, 1).clone(), "encoder_color.embeddings": e["c"].clone(), **mlps}
+        if self.ind_dim:
+            # individual_codes is a parameter of the renderer itself, registered before the network's modules (renderer.py:102)
+            self._with_codes(tensors, e["ind"])
+            order = ["individual_codes"] + order
         return {"decay": self.ema_decay, "num_updates": self.ema_num_updates, "shadow_params": [tensors[k] for k in order],
                 "collected_params": None}
 
@@ -423,6 +503,8 @@ class Stage0Trainer:
         for name, shp in MLP_LAYOUT:
             n = shp[0] * shp[1]
             grads[name] = g[o:o + n].view(shp).clone(); o += n
+        if self.ind_dim:
+            self._with_codes(grads, self.g_ind / self.opt_state[0])
         return grads
 
     def mark_untrained_grid(self, poses, intrinsics, cam_near_far=None):
@@ -459,8 +541,23 @@ class Stage0Trainer:
              ptr(self.ray_ctl) if adaptive else None, self.cfg.num_points if adaptive else 0, stream())
 
     def encode_fwd(self, part=0, nparts=1):
+        if self.ind_dim:
+            call("n2m_s0_encode_fwd_codes", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
+                 ptr(self.table), ptr(self.offsets), self._codes_table(), ptr(self.slots[self.cur].ray_img), ptr(self.enc_tiles), part,
+                 nparts, stream())
+            return
         call("n2m_s0_encode_fwd", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
              ptr(self.table), ptr(self.offsets), ptr(self.enc_tiles), part, nparts, stream())
+
+    def encode_points(self, pp, pts, dirs, counters, cap, enc_tiles, code_row=0):
+        """The hash-grid gather of explicit points pts [cap,3] (dirs nullable; counters[1] points) into tile images with parameter block
+        `pp`; with appearance codes every point reads code row `code_row` (stage 1: the view's image; evaluation and the bake: 0)."""
+        if self.ind_dim:
+            call("n2m_s0_encode_points_codes", pp, ptr(pts), ptr(dirs), ptr(counters), cap, ptr(self.table), ptr(self.offsets),
+                 self.ind.data_ptr() + 4 * self.ind_dim * (64 + int(code_row)), ptr(enc_tiles), stream())
+        else:
+            call("n2m_s0_encode_points", pp, ptr(pts), ptr(dirs), ptr(counters), cap, ptr(self.table), ptr(self.offsets), ptr(enc_tiles),
+                 stream())
 
     def mlp_fwd(self, part=0, nparts=1):
         call("n2m_s0_mlp_fwd", self._pp(), ptr(self.enc_tiles), ptr(self.counters), self.Mcap, ptr(self.wpack), ptr(self.out),
@@ -473,10 +570,27 @@ class Stage0Trainer:
              ptr(self.loss_acc), active, part, nparts, stream())
 
     def mlp_bwd(self, part=0, nparts=1):
+        if self.ind_dim:
+            call("n2m_s0_mlp_bwd_codes", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.Mcap, ptr(self.wpack),
+                 ptr(self.denc_tiles), ptr(self.g_mlp), ptr(self.g_ind), ptr(self.opt_state), part, nparts, stream())
+            self.code_grad(part, nparts)
+            return
         call("n2m_s0_mlp_bwd", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.Mcap, ptr(self.wpack),
              ptr(self.denc_tiles), ptr(self.g_mlp), ptr(self.opt_state), part, nparts, stream())
 
+    def code_grad(self, part=0, nparts=1, all_rays=False):
+        """Gradient of the appearance codes: the code columns of denc_tiles summed per ray into its image's code row."""
+        active = self.counters.data_ptr() + 4 * 16 if self.adaptive and not all_rays else None      # counters[16]: the batch's n
+        call("n2m_s0_code_grad", self._pp(), ptr(self.rays), ptr(self.counters), self.N, ptr(self.denc_tiles),
+             ptr(self.slots[self.cur].ray_img), self.g_ind.data_ptr() + 4 * 64 * self.ind_dim, ptr(self.opt_state), active, part, nparts,
+             stream())
+
     def fwd_fused(self):
+        if self.ind_dim:
+            call("n2m_s0_fwd_fused_codes", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
+                 ptr(self.table), ptr(self.offsets), self._codes_table(), ptr(self.slots[self.cur].ray_img), ptr(self.wpack),
+                 ptr(self.enc_tiles), ptr(self.out), self.loss_acc.data_ptr() + 4, stream())
+            return
         call("n2m_s0_fwd_fused", self._pp(), ptr(self.recs), ptr(self.counters), self.Mcap, ptr(self.rays_o), ptr(self.rays_d),
              ptr(self.table), ptr(self.offsets), ptr(self.wpack), ptr(self.enc_tiles), ptr(self.out), self.loss_acc.data_ptr() + 4, stream())
 
@@ -503,6 +617,8 @@ class Stage0Trainer:
         table (the caller zeroes it off the critical path, see `defer_zero`).  `between`: callable run after the parameter updates and
         before the GradScaler update -- further parameter groups of the same optimizer step (stage 1: the vertex offsets)."""
         main = torch.cuda.current_stream()
+        if self.ind_dim:
+            call("n2m_s0_adam_codes_head", ptr(self.g_ind), self.g_ind.numel(), ptr(self.opt_state), stream())
         call("n2m_s0_adam_head", ptr(self.g_mlp), ptr(self.opt_state), stream())
         if self._adam_stream is None:
             self._adam_stream = torch.cuda.Stream(device=self.device)
@@ -511,6 +627,9 @@ class Stage0Trainer:
         with torch.cuda.stream(side):
             call("n2m_s0_adam_mlp", ptr(self.mlp), ptr(self.g_mlp), ptr(self.m_mlp), ptr(self.v_mlp), ptr(self.wpack),
                  ptr(self.opt_state), self.cfg.eps, stream())
+            if self.ind_dim:        # after adam_mlp, whose weight repack zeroes the code columns
+                call("n2m_s0_adam_codes", ptr(self.ind), ptr(self.g_ind), ptr(self.m_ind), ptr(self.v_ind), self.ind_dim, self.ind_num,
+                     ptr(self.wpack), ptr(self.opt_state), self.cfg.eps, stream())
         call("n2m_s0_adam_tables_keep" if keep_grads else "n2m_s0_adam_tables", ptr(self.table), ptr(self.color_master), ptr(self.gtable),
              ptr(self.m_table), ptr(self.v_table), self.rows, ptr(self.opt_state), self.cfg.eps, stream())
         if between is not None:
@@ -647,7 +766,7 @@ class Stage0Trainer:
             fn()
 
     def step(self, rays_o=None, rays_d=None, gt=None, bg_color=None, noises=None, shading="full", lr=None, use_graph=True,
-             grad_sync=None, next_batch=None, cam_near_far=None):
+             grad_sync=None, next_batch=None, cam_near_far=None, index=None, next_index=None):
         """One optimizer step on the batch (rays_o, rays_d, gt, bg_color[, noises]).
 
         * tensors given: copied into the step buffers first (pinned host -> async H2D);
@@ -659,7 +778,17 @@ class Stage0Trainer:
         * `grad_sync`: callable run between backward and optimizer (data-parallel gradient all-reduce).
         * adaptive ray count (`cfg.adaptive_num_rays`): every batch has `max_rays` (= self.N) rows; the step uses the first n, the count
           the previous march left in `ray_ctl[0]` (recorded in the slot's counters[16]); rows >= n are never read.
+        * `index` (appearance codes, `cfg.ind_dim > 0`: required with a batch, rejected without codes): the reference's data['index'],
+          the training image of the batch (an int) or of every ray (an int32 [N] tensor, random_image_batch).  It is staged with the batch
+          (persistent per-slot buffer: graph replays read it); `next_index` goes with `next_batch`.  Indices on the host are range-checked;
+          a device tensor is not (a check would synchronise, as n2m_s0_gen_rays does not check its indices either).
         No host sync happens here; read `loss_acc` / `counters` afterwards."""
+        self._check_index(index, "index")
+        self._check_index(next_index, "next_index")
+        if self.ind_dim and grad_sync is not None:
+            raise ValueError("data-parallel training with appearance codes (ind_dim > 0) is not supported")
+        if self.ind_dim and next_batch is not None and next_index is None:
+            raise ValueError("next_index is required with next_batch when the model has appearance codes (ind_dim > 0)")
         main = torch.cuda.current_stream()
         if self._prefetched is not None:
             self.cur = self._prefetched
@@ -668,7 +797,11 @@ class Stage0Trainer:
             marched = True
         else:
             if rays_o is not None:
+                if self.ind_dim and index is None:
+                    raise ValueError("index is required when the model has appearance codes (ind_dim > 0)")
                 self.slots[self.cur].load(rays_o, rays_d, gt, bg_color, noises, cam_near_far)
+            if index is not None:
+                self.slots[self.cur].load_index(index)
             marched = False
         if lr is not None:
             self.opt_state[4:5].fill_(float(lr))
@@ -734,6 +867,8 @@ class Stage0Trainer:
             keep = self.cur
             with torch.cuda.stream(side):
                 self.slots[nxt].load(*next_batch)
+                if self.ind_dim:
+                    self.slots[nxt].load_index(next_index)
                 if ev_mid is not None:
                     side.wait_event(ev_mid)
                 if self.adaptive:
@@ -745,6 +880,24 @@ class Stage0Trainer:
                 self._ev_march[nxt] = ev
             self._prefetched = nxt
 
+
+    def _check_index(self, index, what):
+        if index is None:
+            return
+        if not self.ind_dim:
+            raise ValueError(f"{what} given, but the model has no appearance codes (ind_dim = 0)")
+        if isinstance(index, bool) or not isinstance(index, (int, torch.Tensor)):
+            raise ValueError(f"{what} must be an int or an int32 tensor of one index per ray, got {type(index).__name__}")
+        if isinstance(index, torch.Tensor):
+            if index.dtype != torch.int32 or index.shape != (self.N,):
+                raise ValueError(f"{what} must be an int32 tensor of shape ({self.N},), got {index.dtype} {tuple(index.shape)}")
+            if index.device.type != "cpu":
+                return                      # not checked on the device: see step()
+            lo, hi = (int(index.min()), int(index.max())) if index.numel() else (0, 0)
+        else:
+            lo = hi = index
+        if lo < 0 or hi >= self.ind_num:
+            raise ValueError(f"{what} out of range [0, {self.ind_num}): [{lo}, {hi}]")
 
     # -------------------------------------------------------------------------------------------
     # density grid / bitfield update and evaluation rendering
@@ -879,6 +1032,12 @@ class Stage0Trainer:
                  ptr(rb["rays_t"]), ptr(rb["rays_far"]), ptr(rb["alive"]), ptr(rb["ctl"]), ptr(wo), ptr(do), ptr(io), stream())
 
             def rounds(widths):
+                if self.ind_dim:        # evaluation uses code 0 (renderer.py:702-703)
+                    call("n2m_s0_render_rounds_codes", pp, ptr(ro), ptr(rd), ptr(self.density_bitfield), n, widths, len(widths),
+                         ptr(rb["rays_t"]), ptr(rb["rays_far"]), ptr(rb["alive"]), ptr(rb["ctl"]), ptr(rb["recs"]), ptr(rb["enc"]),
+                         ptr(rb["out"]), rb["cap"], ptr(self.table), ptr(self.offsets), ptr(self.wpack), self._codes_table(), ptr(wo),
+                         ptr(do), ptr(io), stream())
+                    return
                 call("n2m_s0_render_rounds", pp, ptr(ro), ptr(rd), ptr(self.density_bitfield), n, widths, len(widths), ptr(rb["rays_t"]),
                      ptr(rb["rays_far"]), ptr(rb["alive"]), ptr(rb["ctl"]), ptr(rb["recs"]), ptr(rb["enc"]), ptr(rb["out"]), rb["cap"],
                      ptr(self.table), ptr(self.offsets), ptr(self.wpack), ptr(wo), ptr(do), ptr(io), stream())
@@ -918,6 +1077,8 @@ class Stage0Trainer:
             if bg is None:
                 bgc = torch.ones(self.N, 3, device=self.device); bgc[:n] = bg_color[a:b]
             slot.load(ro, rd, zeros3, bg if bg is not None else bgc, torch.zeros(self.N, device=self.device))
+            if self.ind_dim:
+                slot.load_index(0)              # evaluation uses code 0 (renderer.py:702-703)
             self.loss_acc.zero_()
             self.march(all_rays=True); self.encode_fwd(); self.mlp_fwd(); self.composite_loss(all_rays=True)
             img[a:b] = self.image[:n]; ws[a:b] = self.weights_sum[:n]; dep[a:b] = self.depth[:n]

@@ -80,6 +80,8 @@ def bg_image(bg_color, q, device):
 class Stage1Trainer:
     v_cumsum = f_cumsum = ()            # per-cascade vertex / face offsets, set by _set_cascades
 
+    _index = 0                  # appearance-code row of the current step's view (t0.ind_dim > 0)
+
     def __init__(self, t0, vertices, triangles, h0, w0, ssaa=2, max_points=None, lambda_mask=0.1, antialias=False, pos_gradient_boost=1.0,
                  lr_vert=0.0, lambda_lap=0.001, lambda_offsets=0.1, refine=False, offset_nerf_grad=False, lambda_normal=0.0, lambda_edgelen=0.0):
         assert ssaa in (1, 2), "the ssaa average equals the reference's bilinear down-scale only at factors 1 and 2"
@@ -216,8 +218,7 @@ class Stage1Trainer:
             call("n2m_s1_points_contract", *pts_args, 1, stream())
         else:
             call("n2m_s1_points", *pts_args, stream())
-        call("n2m_s0_encode_points", self._pp(), ptr(self.pts), ptr(self.pdirs), ptr(self.counters), self.cap, ptr(t0.table),
-             ptr(t0.offsets), ptr(self.enc_tiles), stream())
+        t0.encode_points(self._pp(), self.pts, self.pdirs, self.counters, self.cap, self.enc_tiles, self._index)
         call("n2m_s0_mlp_fwd", self._pp(), ptr(self.enc_tiles), ptr(self.counters), self.cap, ptr(t0.wpack), ptr(self.out), None, 0, 1,
              stream())
         if self.antialias:
@@ -246,8 +247,15 @@ class Stage1Trainer:
             call("n2m_s1_loss_err" if self.refine else "n2m_s1_loss", ptr(self.out), ptr(self.inv), ptr(gt), gt.shape[-1], ptr(bg), self.h0,
                  self.w0, self.ssaa, self.lambda_mask, ptr(t0.opt_state), ptr(self.dout), ptr(self.image), ptr(self.weights_sum),
                  ptr(self.loss_acc), *err, stream())
-        call("n2m_s0_mlp_bwd", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.cap, ptr(t0.wpack),
-             ptr(self.denc_tiles), ptr(t0.g_mlp), ptr(t0.opt_state), 0, 1, stream())
+        if t0.ind_dim:
+            # appearance codes: the view's code row (renderer.py:845-852) gets the summed input gradient of all the view's points
+            call("n2m_s0_mlp_bwd_codes", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.cap, ptr(t0.wpack),
+                 ptr(self.denc_tiles), ptr(t0.g_mlp), ptr(t0.g_ind), ptr(t0.opt_state), 0, 1, stream())
+            call("n2m_s0_code_grad_row", self._pp(), ptr(self.counters), self.cap, ptr(self.denc_tiles),
+                 t0.g_ind.data_ptr() + 4 * t0.ind_dim * (64 + self._index), ptr(t0.opt_state), stream())
+        else:
+            call("n2m_s0_mlp_bwd", self._pp(), ptr(self.enc_tiles), ptr(self.dout), ptr(self.counters), self.cap, ptr(t0.wpack),
+                 ptr(self.denc_tiles), ptr(t0.g_mlp), ptr(t0.opt_state), 0, 1, stream())
         call("n2m_s0_encode_bwd", self._pp(), ptr(self.recs), ptr(self.counters), self.cap, ptr(self.pts), ptr(self.pdirs),
              ptr(self.denc_tiles), ptr(t0.table), ptr(t0.offsets), ptr(t0.gtables[t0.parity]), ptr(t0.opt_state), 0, 1, stream())
         if self.offset_nerf_grad:
@@ -258,12 +266,15 @@ class Stage1Trainer:
                  self.h, self.w, ptr(self.pts), ptr(self.denc_tiles), ptr(t0.table), ptr(t0.offsets), ptr(self.grad_vclip),
                  ptr(self.grad_vworld), ptr(t0.opt_state), stream())
 
-    def step(self, mvp, rays_d, gt, bg, shading="full", lr=None, use_graph=False):
+    def step(self, mvp, rays_d, gt, bg, shading="full", lr=None, use_graph=False, index=None):
         """One optimizer step on one view: mvp [4,4], rays_d [h0*w0,3] (unnormalised), gt [h0*w0, 3 or 4], bg [h0*w0,3].
+        `index` (appearance codes, t0.cfg.ind_dim > 0: required, rejected otherwise): the view's image, data['index'] (utils.py:711);
+        the view's points read its code and the step trains that code (its own Adam group, as in stage 0).
         `use_graph`: the step is captured once per view (keyed by the addresses of its device-resident tensors, which must then stay
         valid and in place -- the dataset of a stage-1 run is a fixed set of views) and replayed as one CUDA graph: ~17 launches and a
         handful of torch ops leave the host's critical path (the eager step is host-bound at this size)."""
         t0 = self.t0
+        self._index = self._check_index(index)
         if lr is not None:
             t0.opt_state[4:5].fill_(float(lr))
         rays_d, gt, bg = rays_d.contiguous(), gt.contiguous(), bg.contiguous()
@@ -275,7 +286,7 @@ class Stage1Trainer:
         else:
             if not (mvp.is_cuda and mvp.dtype == torch.float32 and mvp.is_contiguous()):
                 raise RuntimeError("use_graph: mvp must be a contiguous float32 CUDA tensor that stays in place (the graph is keyed by its address)")
-            key = (mvp.data_ptr(), rays_d.data_ptr(), gt.data_ptr(), bg.data_ptr(), int(gt.shape[-1]), shading, int(t0.parity))
+            key = (mvp.data_ptr(), rays_d.data_ptr(), gt.data_ptr(), bg.data_ptr(), int(gt.shape[-1]), shading, int(t0.parity), self._index)
             g = self._graphs.get(key)
             if g is None:
                 g = torch.cuda.CUDAGraph()
@@ -285,6 +296,20 @@ class Stage1Trainer:
                 g = self._graphs[key]
             g[0].replay()
         t0.global_step += 1
+
+    def _check_index(self, index):
+        t0 = self.t0
+        if not t0.ind_dim:
+            if index is not None:
+                raise ValueError("index given, but the model has no appearance codes (ind_dim = 0)")
+            return 0
+        if index is None:
+            raise ValueError("index is required when the model has appearance codes (ind_dim > 0)")
+        if isinstance(index, bool) or not isinstance(index, int):
+            raise ValueError(f"index must be an int (the view's image), got {type(index).__name__}")
+        if not 0 <= index < t0.ind_num:
+            raise ValueError(f"index {index} out of range [0, {t0.ind_num})")
+        return index
 
     def _step_body(self, mvp, rays_d, gt, bg, shading):
         self.forward(mvp, rays_d, shading)
@@ -365,8 +390,7 @@ class Stage1Trainer:
         rb["rast"] = rast
         call("n2m_s1_points_contract", ptr(rast), ptr(self.vertices), ptr(self.triangles), ptr(rays_d), h, w, self.ssaa, rb["cap"],
              ptr(rb["counters"]), ptr(rb["inv"]), ptr(rb["pts"]), ptr(rb["pdirs"]), ptr(rb["recs"]), int(self.contract), stream())
-        call("n2m_s0_encode_points", pp, ptr(rb["pts"]), ptr(rb["pdirs"]), ptr(rb["counters"]), rb["cap"], ptr(t0.table), ptr(t0.offsets),
-             ptr(rb["enc_tiles"]), stream())
+        t0.encode_points(pp, rb["pts"], rb["pdirs"], rb["counters"], rb["cap"], rb["enc_tiles"], 0)     # inference: code 0 (renderer.py:849-850)
         call("n2m_s0_mlp_fwd", pp, ptr(rb["enc_tiles"]), ptr(rb["counters"]), rb["cap"], ptr(t0.wpack), ptr(rb["out"]), None, 0, 1, stream())
         call("n2m_s1_rgba", ptr(rb["out"]), ptr(rb["inv"]), h * w, ptr(rb["rgba"]), stream())
         img = rb["rgba"]
@@ -461,7 +485,7 @@ class Stage1Trainer:
         self._mesh_buffers()
         if reset_optimizer:
             t0 = self.t0
-            for buf in (t0.m_table, t0.v_table, t0.m_mlp, t0.v_mlp):
+            for buf in (t0.m_table, t0.v_table, t0.m_mlp, t0.v_mlp) + ((t0.m_ind, t0.v_ind) if t0.ind_dim else ()):
                 buf.zero_()
             t0.opt_state[2:3].zero_()
 

@@ -95,8 +95,8 @@ class Baker:
         t0 = self.t0
         call("n2m_s1_bake_points", ptr(rast), ptr(vertices), ptr(triangles), w, y0, y1, self.cap, int(bool(contract)), ptr(self.counters),
              ptr(self.pix), ptr(self.pts), stream())
-        call("n2m_s0_encode_points", t0._pp(), ptr(self.pts), None,
-             ptr(self.counters), self.cap, ptr(t0.table), ptr(t0.offsets), ptr(self.enc_tiles), stream())
+        # with appearance codes the bake uses code 0, as the reference's export does (renderer.py:354-356)
+        t0.encode_points(t0._pp(), self.pts, None, self.counters, self.cap, self.enc_tiles, 0)
 
     def features(self, feats, feats_f32=None):
         """geo_feat of the gathered points, quantised into their texels of feats"""

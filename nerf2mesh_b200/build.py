@@ -17,7 +17,7 @@ OBJ = os.path.join(CSRC, "_obj")
 LIB = os.path.join(HERE, "libn2m_b200.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
-SOURCES = ["raymarching.cu", "gridencoder.cu", "shencoder.cu", "stage0.cu", "mlp_tc.cu", "fused.cu", "render.cu", "mcubes.cu", "cascade.cu", "meshclean.cu", "decimate.cu", "raster.cu", "antialias.cu", "stage1.cu", "texture.cu", "grid_aux.cu", "optim.cu", "dp.cu"]
+SOURCES = ["raymarching.cu", "gridencoder.cu", "shencoder.cu", "stage0.cu", "mlp_tc.cu", "fused.cu", "render.cu", "mcubes.cu", "cascade.cu", "meshclean.cu", "decimate.cu", "atlas.cu", "raster.cu", "antialias.cu", "stage1.cu", "texture.cu", "grid_aux.cu", "optim.cu", "dp.cu"]
 # micro-benchmarks and the wgmma layout probe: test / profiling infrastructure, kept OUT of the product library
 PROBE_SOURCES = ["tc_probe.cu"]
 PROBE_LIB = os.path.join(HERE, "libn2m_probes.so")

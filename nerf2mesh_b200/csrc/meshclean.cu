@@ -21,6 +21,7 @@
 //   k_fan_*                         non-manifold vertices: union-find over face corners joined through an edge at their vertex
 #include "n2m_common.cuh"
 #include "mesh_keys.cuh"
+#include "union_find.cuh"
 #include "../../include/n2m_b200_mesh.h"
 
 #include <limits.h>
@@ -47,32 +48,6 @@ __device__ double box_diag(const uint32_t* lo, const uint32_t* hi) {
 __device__ __forceinline__ double merge_radius(double diag, double v_pct) { return __ddiv_rn(__dmul_rn(__ddiv_rn(v_pct, 100.0), diag), 10.0); }
 // PercentageValue(min_d) of meshing_remove_connected_component_by_diameter read against the whole diagonal
 __device__ __forceinline__ double min_component_diag(double diag, double min_d) { return __dmul_rn(__ddiv_rn(min_d, 100.0), diag); }
-
-// ---- union-find: parent[x] <= x, root = the lowest element of a class ---------------------------------------------------------------
-__device__ int32_t uf_find(int32_t* parent, int32_t x) {
-    volatile int32_t* p = parent;
-    while (true) {
-        const int32_t y = p[x];
-        if (y == x) return x;
-        const int32_t z = p[y];
-        if (z != y) p[x] = z;                  // path halving: z is still an ancestor of x
-        x = y;
-    }
-}
-// once every union is done: the root, without writes (a path-halving write racing a label store could leave a non-root behind)
-__device__ __forceinline__ int32_t uf_root(const int32_t* parent, int32_t x) {
-    int32_t y;
-    while ((y = parent[x]) != x) x = y;
-    return x;
-}
-__device__ void uf_union(int32_t* parent, int32_t a, int32_t b) {
-    while (true) {
-        a = uf_find(parent, a); b = uf_find(parent, b);
-        if (a == b) return;
-        if (a < b) { const int32_t t = a; a = b; b = t; }
-        if (atomicCAS(parent + a, a, b) == a) return;
-    }
-}
 
 __device__ __forceinline__ bool live(const uint8_t* fkeep, uint32_t f) { return fkeep == nullptr || fkeep[f] != 0; }
 

@@ -5,6 +5,11 @@ Host side of csrc/texture.cu (C ABI include/n2m_b200_texture.h).
     export_stage1(s1, save_path, vt, ft, resolution=4096)                 # -> mesh_0.obj, mesh_0.mtl, feat0_0.jpg, feat1_0.jpg, mlp.json
     export_stage1(s1, save_path, [vt0, vt1, ...], [ft0, ft1, ...])       # several cascades: mesh_{cas}.obj ... per cascade, one mlp.json
 
+The UV atlas is the library's own, built on the device (csrc/atlas.cu, C ABI include/n2m_b200_atlas.h) unless the caller passes one:
+    vt, ft, vmapping = uv_unwrap(vertices, triangles, resolution, ssaa=2)   # vmapping[ft] == triangles, as xatlas's vmapping
+    vts, fts = unwrap_stage1(s1, resolution)                                # one unwrap per cascade mesh (of contract(v) when cfg.contract)
+    export_stage1(s1, save_path, resolution=4096)                           # unwrap_stage1, then the bake and the files
+
 The stages, each callable on its own:
     uv_features(t0, vertices, triangles, vt, ft, h, w)  UV raster (n2m_rasterize of (vt * 2 - 1, 0, 1) / ft), positions interpolated with
                                                         the position triangles, hash-grid gather, geo_feat on tensor cores, quantised:
@@ -24,7 +29,10 @@ Looking at the result -- what the viewer (renderer.html) shows, and how much the
 render_exported rasterizes every cascade into one depth buffer and runs the viewer's fragment shader on the device (n2m_s1_asset_shade:
 nearest texel, specular_net in fp32), then the evaluation compose of Stage1Trainer.render.
 """
+import ctypes
+import itertools
 import json
+import math
 import os
 
 import numpy as np
@@ -33,7 +41,8 @@ import torch
 from . import _lib
 from . import raster as dr
 from . import stage0  # noqa: F401  (binds the stage-0 gather n2m_s0_encode_points)
-from ._lib import F, P, U, call, ptr, stream
+from . import mesh as _mesh  # noqa: F401  (binds n2m_clean_edge_table)
+from ._lib import F, I, P, U, call, ptr, stream
 
 _lib.register({
     "n2m_s1_bake_points": [P, P, P, U, U, U, U, U, P, P, P, P],
@@ -41,6 +50,20 @@ _lib.register({
     "n2m_s1_inpaint": [P, P, U, U, P, P, P],
     "n2m_s1_ssaa_down2": [P, U, U, U, P, P, P],
     "n2m_s1_asset_shade": [P, U, P, P, P, P, P, U, P, P, P, P, F, F, F, U, P, P],
+    "n2m_atlas_contract": [P, U, P, P],
+    "n2m_atlas_faces": [P, P, U, P, P, P, P, P],
+    "n2m_atlas_base": [U, P, P, P, P, U, P, P, P, P, P, P, P],
+    "n2m_atlas_chart_count": [U, P, P, P],
+    "n2m_atlas_merge_round": [U, U, P, P, P, P, P, P, P, P, P, P, P, P],
+    "n2m_atlas_roots": [U, P, P, P],
+    "n2m_atlas_orient": [P, P, U, P, P, P, P, P, U, U, P, P, P, P, P, P, P, P],
+    "n2m_atlas_sort": [P, P, U, U, P],
+    "n2m_atlas_pack": [P, P, U, I, I, I, P, P, P, P, P, P, P, P, P],
+    "n2m_atlas_conflicts": [P, P, U, P, P, P, P, P, P, P, P, P, P, U, I, U, P, P, P, P],
+    "n2m_atlas_split": [U, U, P, P, P, P, P, P, P, P],
+    "n2m_atlas_corner_keys": [P, U, P, P, P, P, P],
+    "n2m_atlas_row_flags": [P, U, P, P],
+    "n2m_atlas_emit": [P, P, P, U, P, P, P, P, P, P, P, P, I, P, P, P, P],
 })
 
 MAX_BAND_POINTS = 1 << 22          # points per band: 512 MiB of gather tiles (128 B per point) + 64 MiB of positions and texel indices
@@ -175,6 +198,192 @@ def bake_features(t0, vertices, triangles, vt, ft, h0, w0, ssaa=2, band_rows=Non
     return downscale(feats, ssaa)
 
 
+# ---- the UV atlas (csrc/atlas.cu) ----------------------------------------------------------------------------------------------------
+# The atlas rule's constants (see uv_unwrap).  At resolution 512 they give 26 charts on icosphere(4) and on the 64^3 marching-cubes
+# sphere, 50 on the 64^3 torus, and 897 on the 2,179 faces of the seeded noisy sphere decimated to 10 %, whose rough charts split into
+# single faces (tests/test_atlas_cpu.py).
+SMALL_CHART = 8          # a chart of fewer faces is small and may merge into a neighbour
+MERGE_ROUNDS = 3         # merge rounds
+ANGLES = 16              # in-plane rotations k * 90 deg / ANGLES tried per chart
+PAD = 2                  # final texels between charts and to the border
+BISECT_STEPS = 24        # geometric bisection steps of the common scale over [hi 2^-20, hi]
+MERGE_COS = 0.5          # a small chart's faces must all be within 60 deg of the target's axis (the kernel's constant, stated here)
+
+
+def atlas_tables():
+    """(axes [26,3], basis [26,6], rot [ANGLES,2]) float64: the 26 directions normalize(i, j, k), (i, j, k) in {-1, 0, 1}^3 \\ 0 in
+    lexicographic order; per axis a right-handed in-plane basis e1 = normalize(cross(h, a)), e2 = cross(a, e1) with h = (0, 0, 1), or
+    (1, 0, 0) for the two z axes; (cos, sin) of k * (pi / 2) / ANGLES"""
+    dirs = np.array([d for d in itertools.product((-1.0, 0.0, 1.0), repeat=3) if any(d)], np.float64)
+    axes = dirs / np.sqrt((dirs * dirs).sum(1))[:, None]
+    basis = np.empty((26, 6), np.float64)
+    for i, a in enumerate(axes):
+        h = np.array([1.0, 0.0, 0.0]) if abs(a[2]) == 1.0 else np.array([0.0, 0.0, 1.0])
+        e1 = np.cross(h, a)
+        e1 = e1 / np.sqrt(e1 @ e1)
+        basis[i, :3], basis[i, 3:] = e1, np.cross(a, e1)
+    t = np.arange(ANGLES, dtype=np.float64) * (math.pi / 2) / ANGLES
+    return axes, basis, np.stack([np.cos(t), np.sin(t)], 1)
+
+
+_atlas_tables = {}
+
+
+def _device_atlas_tables(device):
+    key = torch.device(device).index
+    if key not in _atlas_tables:
+        _atlas_tables[key] = tuple(torch.from_numpy(np.ascontiguousarray(x)).to(device) for x in atlas_tables())
+    return _atlas_tables[key]
+
+
+def _pow2(n):
+    return 1 << max(int(n) - 1, 1).bit_length()
+
+
+@torch.no_grad()
+def uv_unwrap(vertices, triangles, resolution, ssaa=2, info=None):
+    """The library's UV atlas of a mesh on the device: vertices [V,3] float32, triangles [F,3] int32 -> (vt [Nt,2] float32, ft [F,3] int32,
+    vmapping [Nt] int32), all CUDA, with vmapping[ft] == triangles.  The atlas is laid out for a `resolution`^2 texture baked at
+    R = resolution * ssaa.  This is a deterministic rule of its own, not xatlas's:
+
+    1. each face's float64 unit normal picks the nearest of 26 axes (the cube's faces, edges and corners; the lowest on a tie), so it
+       lies within about 27.6 deg of it: projection stretches area by at most 1.13x and flips no face.  A face that repeats an index or
+       whose cross product is zero is a chart of its own (it covers no texel);
+    2. faces across an edge of exactly two faces with the same axis share a base chart;
+    3. MERGE_ROUNDS rounds: a chart of fewer than SMALL_CHART faces merges into the neighbour it shares the most such edges with (ties:
+       the lowest chart id) when all its faces are within 60 deg of that chart's axis and that chart is not merging itself; the merged
+       chart keeps the target's axis;
+    4. each chart is projected onto its axis's plane and turned by the one of ANGLES angles that gives the least bounding box, then by
+       90 deg when the box is taller than wide;
+    5. one scale s (final texels per unit length) for every chart: the largest, by bisection, at which next-fit-decreasing-height shelves
+       of the charts' ceil(s w) x ceil(s h) rectangles fit, PAD final texels apart and from the border -- on the final texel grid, so no
+       texel of the down-sampled texture mixes two charts;
+    6. a chart in which two faces cover the same bake-raster texel centre (strictly inside both) splits into its base charts when it is
+       a merged chart, else into single faces, and the packing runs again.  A new scale samples the charts anew, so a chart clear at
+       one scale may conflict at the next; every split lowers a chart's level (merged, base, single face) and single faces in their own
+       rectangles cannot conflict, so the rounds end;
+    7. vt has one row per distinct (chart, vertex) in that order, vt = (offset + s * xy) / resolution rounded once to float32.
+
+    `info`, a dict, receives `charts`, `texels_per_unit` (s), `utilization` (the UV area of the faces, of 1) and `split_rounds`.  ValueError
+    for malformed input, a bake raster of 2^31 texels or more, or charts that do not fit the texture even at the smallest scale."""
+    if not (torch.is_tensor(vertices) and torch.is_tensor(triangles) and vertices.is_cuda):
+        raise ValueError("uv_unwrap: vertices and triangles must be tensors, the vertices on a CUDA device")
+    if vertices.dim() != 2 or vertices.shape[1] != 3 or triangles.dim() != 2 or triangles.shape[1] != 3:
+        raise ValueError("uv_unwrap: vertices [V,3] and triangles [F,3]")
+    if vertices.dtype != torch.float32 or triangles.dtype not in (torch.int32, torch.int64):
+        raise ValueError("uv_unwrap: vertices must be float32 and triangles int32 or int64")
+    resolution, ssaa = int(resolution), int(ssaa)
+    R = resolution * ssaa
+    if ssaa < 1 or resolution <= 2 * PAD or R * R >= 1 << 31:
+        raise ValueError(f"uv_unwrap: texture {resolution} x ssaa {ssaa}: the texture exceeds {2 * PAD} texels and the bake raster holds "
+                         "fewer than 2^31 texels")
+    dev = vertices.device
+    V, Fn = int(vertices.shape[0]), int(triangles.shape[0])
+    if 3 * Fn >= 1 << 31:
+        raise ValueError("uv_unwrap: at most 2^31 / 3 faces")
+    v = vertices.contiguous()
+    tri = triangles.to(dev, torch.int32).contiguous()
+    if Fn and (int(triangles.min()) < 0 or int(triangles.max()) >= V):
+        raise ValueError(f"uv_unwrap: triangles index outside the vertices (0..{V - 1})")
+    if V and not bool(torch.isfinite(v).all()):
+        raise ValueError("uv_unwrap: vertices must be finite")
+    i32 = dict(dtype=torch.int32, device=dev)
+    if Fn == 0:
+        if info is not None:
+            info.update(charts=0, texels_per_unit=0.0, utilization=0.0, split_rounds=0)
+        return torch.empty(0, 2, device=dev), torch.empty(0, 3, **i32), torch.empty(0, **i32)
+    axes, basis, rot = _device_atlas_tables(dev)
+    nrm = torch.empty(Fn, 3, dtype=torch.float64, device=dev)
+    bucket, fkeep = torch.empty(Fn, **i32), torch.empty(Fn, dtype=torch.uint8, device=dev)
+    call("n2m_atlas_faces", ptr(v), ptr(tri), Fn, ptr(axes), ptr(nrm), ptr(bucket), ptr(fkeep), stream())
+    ne = _pow2(6 * Fn)                                                       # 2. base charts
+    table, slot_of, ecount, mate = torch.empty(ne, **i32), torch.empty(3 * Fn, **i32), torch.empty(ne, **i32), torch.empty(3 * Fn, **i32)
+    call("n2m_clean_edge_table", ptr(tri), Fn, ptr(fkeep), ne, ptr(table), ptr(slot_of), stream())
+    parent, base, label, fax = (torch.empty(Fn, **i32) for _ in range(4))
+    call("n2m_atlas_base", Fn, ptr(fkeep), ptr(bucket), ptr(table), ptr(slot_of), ne, ptr(ecount), ptr(mate), ptr(parent), ptr(base),
+         ptr(label), ptr(fax), stream())
+    del table, slot_of, ecount, parent
+    count, start, cursor, items, propose = (torch.empty(Fn, **i32) for _ in range(5))
+    for _ in range(MERGE_ROUNDS):                                            # 3. small charts
+        call("n2m_atlas_chart_count", Fn, ptr(label), ptr(count), stream())
+        torch.cumsum(count, 0, dtype=torch.int32, out=start)
+        start -= count
+        call("n2m_atlas_merge_round", Fn, SMALL_CHART, ptr(nrm), ptr(axes), ptr(bucket), ptr(mate), ptr(count), ptr(start), ptr(cursor),
+             ptr(items), ptr(propose), ptr(label), ptr(fax), stream())
+    del count, start, cursor, items, propose, mate, nrm
+    owner = torch.empty(R * R, **i32)
+    nconf, state = torch.empty(1, **i32), torch.empty(2, dtype=torch.float64, device=dev)
+    splits = 0
+    while True:
+        flag = torch.empty(Fn, **i32)                                        # chart indices
+        call("n2m_atlas_roots", Fn, ptr(label), ptr(flag), stream())
+        incl = torch.cumsum(flag, 0, dtype=torch.int32)
+        C = int(incl[-1].item())                                             # read-back: the chart count
+        cap = _pow2(C)
+        bmin, bmax = torch.empty(C * ANGLES * 2, dtype=torch.int64, device=dev), torch.empty(C * ANGLES * 2, dtype=torch.int64, device=dev)
+        orient, org, ext = torch.empty(C, **i32), torch.empty(C, 2, dtype=torch.float64, device=dev), torch.empty(C, 2, dtype=torch.float64, device=dev)
+        skey, sval = torch.empty(cap, dtype=torch.int64, device=dev), torch.empty(cap, **i32)
+        call("n2m_atlas_orient", ptr(v), ptr(tri), Fn, ptr(label), ptr(incl), ptr(fax), ptr(basis), ptr(rot), ANGLES, C, ptr(bmin), ptr(bmax),
+             ptr(orient), ptr(org), ptr(ext), ptr(skey), ptr(sval), stream())
+        del bmin, bmax
+        call("n2m_atlas_sort", ptr(skey), ptr(sval), C, cap, stream())     # 5. packing
+        wid, hgt, nxt, shelf_a, shelf_y = (torch.empty(C, **i32) for _ in range(5))
+        prefix, off = torch.empty(C + 1, dtype=torch.int64, device=dev), torch.empty(C, 2, **i32)
+        call("n2m_atlas_pack", ptr(ext), ptr(sval), C, resolution, PAD, BISECT_STEPS, ptr(wid), ptr(hgt), ptr(nxt), ptr(shelf_a), ptr(shelf_y),
+             ptr(prefix), ptr(off), ptr(state), stream())
+        del wid, hgt, nxt, shelf_a, shelf_y, prefix, skey, sval
+        scale, fits = state.tolist()                                         # read-back: the scale and whether the charts fit
+        if not fits:
+            raise ValueError(f"uv_unwrap: {C} charts do not fit a {resolution}^2 texture even at the smallest scale; use a larger resolution")
+        conf = torch.empty(C, dtype=torch.uint8, device=dev)                 # 6. texel conflicts
+        call("n2m_atlas_conflicts", ptr(v), ptr(tri), Fn, ptr(fkeep), ptr(label), ptr(incl), ptr(fax), ptr(basis), ptr(rot), ptr(orient),
+             ptr(org), ptr(off), ptr(state), C, resolution, R, ptr(owner), ptr(conf), ptr(nconf), stream())
+        if int(nconf.item()) == 0:                                           # read-back: the conflict count
+            break
+        merged = torch.empty(C, dtype=torch.uint8, device=dev)
+        call("n2m_atlas_split", Fn, C, ptr(incl), ptr(base), ptr(bucket), ptr(conf), ptr(merged), ptr(label), ptr(fax), stream())
+        splits += 1
+    del owner
+    cap = _pow2(3 * Fn)                                                      # 7. emit
+    keys, vals = torch.empty(cap, dtype=torch.int64, device=dev), torch.empty(cap, **i32)
+    call("n2m_atlas_corner_keys", ptr(tri), Fn, ptr(label), ptr(incl), ptr(keys), ptr(vals), stream())
+    call("n2m_atlas_sort", ptr(keys), ptr(vals), 3 * Fn, cap, stream())
+    rows = torch.empty(3 * Fn, **i32)
+    call("n2m_atlas_row_flags", ptr(keys), 3 * Fn, ptr(rows), stream())
+    torch.cumsum(rows, 0, dtype=torch.int32, out=rows)
+    Nt = int(rows[-1].item())                                                # read-back: the row count
+    vt, ft, vmapping = torch.empty(Nt, 2, device=dev), torch.empty(Fn, 3, **i32), torch.empty(Nt, **i32)
+    call("n2m_atlas_emit", ptr(v), ptr(keys), ptr(vals), 3 * Fn, ptr(rows), ptr(fax), ptr(basis), ptr(rot), ptr(orient), ptr(org), ptr(off),
+         ptr(state), resolution, ptr(vt), ptr(ft), ptr(vmapping), stream())
+    if info is not None:
+        info.update(charts=C, texels_per_unit=scale, utilization=uv_area(vt, ft), split_rounds=splits)
+    return vt, ft, vmapping
+
+
+def uv_area(vt, ft):
+    """the summed float64 area of the UV triangles (of the unit square)"""
+    t = vt.double()[ft.long()]
+    d1, d2 = t[:, 1] - t[:, 0], t[:, 2] - t[:, 0]
+    return float((0.5 * (d1[:, 0] * d2[:, 1] - d1[:, 1] * d2[:, 0]).abs()).sum())
+
+
+def unwrap_stage1(s1, resolution):
+    """uv_unwrap of every cascade mesh of a Stage1Trainer (s1.cascade_mesh(cas)) for its texture size texture_sizes(resolution, C)[cas] and
+    the trainer's ssaa, of the contracted positions when the trainer's cfg.contract (renderer.py:314); the bake itself reads the
+    uncontracted ones.  -> (vts, fts): one vt [Nt,2] and ft [F,3] per cascade."""
+    vts, fts = [], []
+    for cas, size in enumerate(texture_sizes(resolution, s1.cascades)):
+        v, f = s1.cascade_mesh(cas)
+        v = v.float().contiguous()
+        if s1.t0.cfg.contract:
+            out = torch.empty_like(v)
+            call("n2m_atlas_contract", ptr(v), int(v.shape[0]), ptr(out), stream())
+            v = out
+        vt, ft, _ = uv_unwrap(v, f, size, ssaa=s1.ssaa)
+        vts.append(vt); fts.append(ft)
+    return vts, fts
+
+
 # ---- files ----------------------------------------------------------------------------------------------------------------------
 def _np(x, dtype):
     if torch.is_tensor(x):
@@ -241,16 +450,23 @@ def texture_sizes(resolution, cascades):
     return sizes
 
 
-def export_stage1(s1, save_path, vt, ft, resolution=4096, band_rows=None):
+def export_stage1(s1, save_path, vt=None, ft=None, resolution=4096, band_rows=None):
     """NeRFRenderer.export_stage1 from a Stage1Trainer (renderer.py:298-468): for every cascade `cas` of the trainer, its mesh
     (s1.cascade_mesh(cas): vertices = base + offsets), the model of its Stage0Trainer (call t0.ema_apply() first to export the EMA
     parameters) and the trainer's ssaa give mesh_{cas}.obj, mesh_{cas}.mtl, feat0_{cas}.jpg, feat1_{cas}.jpg under save_path; then mlp.json
-    with `cascade` = the number of cascades.  vt [Nt,2] / ft [F,3] come from the caller's UV unwrap of the mesh (of contract(vertices) when
-    cfg.contract, renderer.py:314); a trainer of several cascades takes lists vt[cas] / ft[cas], one unwrap per cascade.  The texture is
+    with `cascade` = the number of cascades.  Without vt / ft the atlas is the library's (unwrap_stage1, one uv_unwrap per cascade).
+    Otherwise vt [Nt,2] / ft [F,3] come from the caller's UV unwrap of the mesh (of contract(vertices) when cfg.contract, renderer.py:314);
+    a trainer of several cascades takes lists vt[cas] / ft[cas], one unwrap per cascade.  The texture is
     `resolution` for cascade 0 and halves after each cascade while it is > 2048 (texture_sizes).  Returns (feat0, feat1) on the device for
     one mesh, the list of them per cascade for lists."""
     t0 = s1.t0
     C = s1.cascades
+    if (vt is None) != (ft is None):
+        raise ValueError("export_stage1: pass both vt and ft, or neither (the library's atlas)")
+    if vt is None:
+        vt, ft = unwrap_stage1(s1, resolution)
+        if C == 1:
+            vt, ft = vt[0], ft[0]
     per_cascade = isinstance(vt, (list, tuple))
     vts, fts = (list(vt), list(ft)) if per_cascade else ([vt], [ft])
     if len(vts) != C or len(fts) != C:
